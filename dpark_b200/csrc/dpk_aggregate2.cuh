@@ -221,9 +221,9 @@ __device__ __forceinline__ uint32_t ag2_slot(const uint32_t (&slots)[3], int j) 
 
 // CURSOR = true (default): the output range of a fine bucket inside its partition is reserved with ONE
 // atomicAdd on the partition's count (the buckets of a partition come out in any order: a reduce partition is a
-// set).  CURSOR = false: the round-1 scheme, a chained scan with decoupled look-back over fb_state[] (deterministic
-// order).  With hundreds of resident CTAs all finishing equal-sized buckets in lockstep, the look-back waits for
-// the SLOWEST of its nearest predecessors every time, and a wider look-back window does not help; the atomic costs a fixed L2 round trip, no waiting on other CTAs, and lifts the
+// set).  CURSOR = false: the round-1 scheme, a chained scan with decoupled look-back over fb_state[] (fine buckets in
+// order; the rows inside one still come in run-to-run varying order, as the unordered multisplits deliver them).
+// With hundreds of resident CTAs all finishing equal-sized buckets in lockstep, the look-back waits for the SLOWEST of its nearest predecessors every time, and a wider look-back window does not help; the atomic costs a fixed L2 round trip, no waiting on other CTAs, and lifts the
 // in-order requirement, so the next ticket and its row range are prefetched a bucket ahead.
 template <typename KeyT, typename ValT, typename AccT, int MINB, bool CURSOR, bool BATCHED, bool FAST_ONLY = false>
 __global__ void __launch_bounds__(AG2_THREADS, MINB)

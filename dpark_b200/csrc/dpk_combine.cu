@@ -106,7 +106,9 @@ template <> struct Acc<double> {
         case DPK_OP_MIN: d = INFINITY; break;
         case DPK_OP_MAX: d = -INFINITY; break;
         case DPK_OP_PROD: d = 1.0; break;
-        default: d = 0.0;
+        // SUM: -0.0 + x is bitwise x for every x (+0.0 + -0.0 would be +0.0), so an accumulator that starts at the
+        // identity ends where one seeded with the first value does: a key whose values are all -0.0 sums to -0.0
+        default: d = -0.0;
         }
         int64_t b;
         memcpy(&b, &d, 8);
@@ -217,15 +219,18 @@ k_tbl_init(Slot *__restrict__ table, const int64_t *__restrict__ tbl_total, int6
     for (; i < slots; i += stride) reinterpret_cast<int4 *>(table)[i] = fill;
 }
 
+// n is the length of the buffer; *rows_total (k_tbl_plan's part_off[nparts]) the rows seg_rows describes, the only
+// ones the table regions are sized for
 template <typename KeyT, typename ValT, typename AccT>
 __global__ void __launch_bounds__(CB_THREADS)
 k_tbl_insert(const KeyT *__restrict__ keys, const int64_t *__restrict__ aux, const ValT *__restrict__ vals,
-             int64_t n, int op, PartFn f, int32_t bucket_first, int32_t F,
+             int64_t n, const int64_t *__restrict__ rows_total, int op, PartFn f, int32_t bucket_first, int32_t F,
              const int64_t *__restrict__ tbl_off, Slot *__restrict__ table, Slot *__restrict__ side,
              int32_t *__restrict__ side_used) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) {
+    const int64_t rows = min(n, *rows_total);
+    for (; i < rows; i += stride) {
         const KeyT key = keys[i];
         const int64_t kb = key_bits<KeyT>(key);
         const AccT v = (AccT)vals[i];
@@ -444,7 +449,6 @@ static inline int grid_cap(int64_t items, int per_cta, int waves) {
 
 int g_reduce_impl = 2;  // dpk_set_option("reduce_impl", 0|1|2)
 
-constexpr int AG_MAX_SB2 = 10;       // at most 1024 fine buckets per first-level bucket
 int g_agg_wide = 1;
 int g_agg_ctas = 4;                  // 4 resident CTAs (64 registers, some spills): H100 C2 merge 1.70 ms vs 1.92 ms at 3
 int g_agg_timing = 0;
@@ -456,12 +460,6 @@ int g_agg_impl = 1;                  // dpk_set_option("agg_impl"): 1 = k_smem_a
 int g_agg_target_rows = 2048;        // rows per fine bucket the split aims for (H100, C4: a 1536 target costs more --
                                      // 6.7 ms merge + 12.2 ms second-level split, 32.2 ms per step -- than 2048 with part
                                      // of the buckets in the multi-window path: 3.4 + 3.3 + 8.4 ms, 28.2 ms per step)
-
-static inline int choose_sb2(int64_t n, int32_t F) {
-    int sb2 = 0;
-    while (sb2 < AG_MAX_SB2 && n / ((int64_t)F << sb2) > g_agg_target_rows) sb2++;
-    return sb2;
-}
 
 struct Ctx {
     int key_kind, val_bytes;
@@ -493,10 +491,10 @@ static int dispatch_op(const Ctx &c) {
     const int64_t ident = Acc<AccT>::identity(c.op);
     if (g_reduce_impl == 2) {
         // second-level split into the (idle) table region, then shared-memory merge per fine bucket
-        const int sb2 = choose_sb2(c.n, c.F);
+        const int sb2 = choose_sb2(c.n, c.F, g_agg_target_rows);
         const int32_t S2 = 1 << sb2;
-        PartFn fine = c.f;
-        fine.mode = 5; fine.P = S2; fine.shift = 32 - c.f.sub_bits - sb2; fine.sub_bits = 0; fine.row_hash = c.aux;
+        PartFn fine = fine_partfn(c.f, sb2);
+        fine.row_hash = c.aux;
         KeyT *rekeys = (KeyT *)c.table;
         ValT *revals = (ValT *)((char *)c.table + (size_t)c.n * 8);
         int rc = seg_multisplit(c.keys, c.key_kind, c.vals, (int32_t)sizeof(ValT), c.n, fine, c.F, c.nsrc, c.seg_start,
@@ -606,7 +604,8 @@ static int dispatch_op(const Ctx &c) {
             c.table, c.tbl_off + c.F, ident));
         if (c.n > 0) {
             DPK_LAUNCH("tbl_insert", c.st, k_tbl_insert<KeyT, ValT, AccT><<<grid_cap(c.n, CB_THREADS, 16), CB_THREADS, 0, c.st>>>(
-                (const KeyT *)c.keys, c.aux, (const ValT *)c.vals, c.n, c.op, c.f, c.part_first << c.f.sub_bits,
+                (const KeyT *)c.keys, c.aux, (const ValT *)c.vals, c.n, c.part_off + c.nparts, c.op, c.f,
+                c.part_first << c.f.sub_bits,
                 c.F, c.tbl_off, c.table, c.side, c.side_used));
         }
         size_t sh = (size_t)((c.nparts + 1) & ~1) * 4 + (size_t)c.nparts * 8;
@@ -645,7 +644,7 @@ static int run_combine(Ctx &c, int val_kind, int64_t *out_offsets, void *ws) {
     c.part_off = out_offsets;
     // implementation 2: fine_off[F * 256 + 1] | segmented-multisplit workspace
     c.fine_off = seg_start + (int64_t)c.nsrc * c.F + 2;
-    const int sb2 = choose_sb2(c.n, c.F);
+    const int sb2 = choose_sb2(c.n, c.F, g_agg_target_rows);
     c.fb_state = (unsigned long long *)(c.fine_off + ((int64_t)c.F << sb2) + 2);
     c.part_err = (int *)(c.fb_state + ((int64_t)c.F << sb2) + 2);
     c.seg_ws = (void *)(((uintptr_t)(c.part_err + c.F + 2) + 255) & ~(uintptr_t)255);
@@ -776,8 +775,8 @@ int64_t dpk_combine_workspace_bytes(int64_t n, int32_t nbuckets, int32_t nsrc) {
     if (nsrc < 1) nsrc = 1;
     return (max_slots_for(n, nbuckets) + 2) * (int64_t)sizeof(Slot) +
            ((int64_t)nbuckets + 4 + (int64_t)nbuckets * nsrc) * 8 + 64 +
-           (((int64_t)nbuckets << choose_sb2(n, nbuckets)) + 4) * 16 + 512 + ((int64_t)nbuckets + 2) * 4 +
-           seg_multisplit_ws_bytes(n, nbuckets, 1 << choose_sb2(n, nbuckets), nsrc);
+           (((int64_t)nbuckets << choose_sb2(n, nbuckets, g_agg_target_rows)) + 4) * 16 + 512 + ((int64_t)nbuckets + 2) * 4 +
+           seg_multisplit_ws_bytes(n, nbuckets, 1 << choose_sb2(n, nbuckets, g_agg_target_rows), nsrc);
 }
 
 int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const void *vals, int val_kind, int64_t n,

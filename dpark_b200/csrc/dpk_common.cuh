@@ -248,6 +248,22 @@ DPK_HD uint32_t slot_hash32(uint64_t kb) {
     return x;
 }
 
+// Second-level split of the reduce side (dpk_combine.cu, implementation 2): every one of the F first-level buckets
+// of n rows is split 2^sb2 ways (PartFn mode 5) until the average fine bucket holds at most target_rows rows
+// (dpk_set_option "agg_target_rows"), at most 2^AG_MAX_SB2 ways.
+constexpr int AG_MAX_SB2 = 10;
+DPK_HD int choose_sb2(int64_t n, int32_t F, int target_rows) {
+    int sb2 = 0;
+    while (sb2 < AG_MAX_SB2 && n / ((int64_t)F << sb2) > target_rows) sb2++;
+    return sb2;
+}
+// the functor of that split: fine bucket = the 2^sb2 bits of mixed(hash) below the first level's sub_bits
+DPK_HD PartFn fine_partfn(const PartFn &first, int sb2) {
+    PartFn fine = first;
+    fine.mode = 5; fine.P = 1 << sb2; fine.shift = 32 - first.sub_bits - sb2; fine.sub_bits = 0;
+    return fine;
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

@@ -211,9 +211,10 @@ int dpk_fused_plan(const int64_t *all_counts, int32_t nranks, int32_t nbuckets, 
  * Accumulation: I64/I32 values -> int64 (exact while |sum| < 2^63, like the
  * reference's big ints); F64/F32 values -> float64 (the reference adds Python
  * floats); out_vals is 8 bytes per row.  out_keys/out_vals hold n entries.
- * n may be an UPPER BOUND of the rows (e.g. the capacity of a receive buffer): with the
- * default reduce_impl 2 only the rows seg_rows describes are read, so a multi-GPU caller
- * needs no host read of the received row count.
+ * n may be an UPPER BOUND of the rows (e.g. the capacity of a receive buffer): every
+ * reduce_impl reads only the rows seg_rows describes, so a multi-GPU caller needs no host
+ * read of the received row count.
+ * Float sums start from -0.0, so a key whose only values are -0.0 sums to -0.0 as in Python.
  * Errors that only the device can see: out_counts[j] == -1 marks a partition whose merge
  * failed -- a fine bucket held more distinct keys than the shared-memory table takes even
  * after splitting it by every spare hash bit (dpk_aggregate2.cuh); nothing is dropped
@@ -225,7 +226,8 @@ int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const vo
                 int32_t sub_bits, int32_t part_first, int32_t nparts, int32_t nsrc,
                 const int64_t *seg_rows, void *out_keys, void *out_vals, int64_t *out_offsets,
                 int64_t *out_counts, void *ws, int64_t ws_bytes, dpk_stream_t stream);
-/* Process-wide A/B switches (results are identical for every setting; only the speed differs):
+/* Process-wide A/B switches (results are the same for every setting -- the same set of rows per reduce partition,
+ * float sums within their rounding; only the speed differs):
  *   "reduce_impl"     2 (default) second-level split + one CTA per fine bucket merging in a
  *                     shared-memory table; 1 = per-bucket tables in HBM, one 8-CTA cluster per bucket;
  *                     0 = three grid-wide passes over global tables
@@ -233,7 +235,7 @@ int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const vo
  *                     cas.b32; 0 = the round-1 kernel (128-bit {key, accumulator} slots)
  *   "agg_cursor"      1 (default) a fine bucket reserves its output range with one atomicAdd on the
  *                     partition's count (partitions are sets: any order); 0 = chained scan with
- *                     decoupled look-back (deterministic order)
+ *                     decoupled look-back (fine buckets in order; the order inside one still varies)
  *   "agg_batched"     1 = four rows per thread in flight in the insert phase; 0 (default) = probe loop per row
  *   "agg_ctas"        4 (default) or 3 resident CTAs per SM the merge kernel is compiled for
  *   "agg_pipe"        0 (default); 1 = k_smem_aggregate3 (rows stay in registers, next bucket prefetched: faster on
@@ -248,7 +250,15 @@ int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const vo
  *                     staged tile through cp.async.bulk (TMA, SASS UBLKCP); 0 = the round-1 kernel
  *   "scatter_threads" 512 (default), 256 or 1024 threads per CTA of the bulk kernel (1024: 8192-row tiles)
  *   "scatter_seg_wide" 1 (default): the segmented (second-level) launches use the 1024-thread form
- *   "scatter_items"   round-1 kernel only: 16 (default) or 8 rows per thread and tile */
+ *   "scatter_wide_from" 512 (default): bucket count from which plain bulk launches use 8192-row tiles (0 = never)
+ *   "scatter_ptr_bulk" 1 (default): unordered pointer-mode scatters (dpk_partition_scatter_ptrs) run the bulk
+ *                     kernel; 0 = the round-1 kernel
+ *   "scatter_ptr_threads" 1024 (default) or 512 threads per CTA of the bulk kernel in pointer mode
+ *   "scatter_items"   round-1 kernel only: 16 (default) or 8 rows per thread and tile
+ *   "agg_split"       1 (default): the one-window buckets and the oversized ones take separate launches
+ *   "copy_sms"        0 (default) = dpk_copy_segments fills the GPU; n > 0 = it runs on n whole SMs
+ *   "copy_tma"        1 (default): copies on a few SMs run through the TMA; 0 = loads and stores
+ *   "agg_timing"      0 (default); 1 = debugging aid: the merge kernel prints its per-phase cycle counts */
 int dpk_set_option(const char *name, int64_t value);
 
 /* ---- a10: reduce side of groupByKey (dpark/dependency.py:107-118 merged by

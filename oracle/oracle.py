@@ -153,6 +153,21 @@ def partition_vec(hashes, P, thresholds=None):
     return out
 
 
+def _key_bits(keys):
+    """int64 identity of a key column for the C loops: integers widened; floats keyed by the bits of their
+    canonical float64 (`arr + 0.0`: -0.0 and 0.0 are one Python dict key, spelled 0.0, as dpark_b200/columnar.py
+    does), so distinct floats stay distinct keys."""
+    keys = np.asarray(keys)
+    if keys.dtype.kind == "f":
+        return np.ascontiguousarray(keys.astype(np.float64) + 0.0).view(np.int64)
+    return np.ascontiguousarray(keys, dtype=np.int64)
+
+
+def _keys_from_bits(bits, dtype):
+    """Inverse of _key_bits for the keys a C loop returns: floats come back in their input dtype."""
+    return bits.view(np.float64).astype(dtype) if dtype.kind == "f" else bits
+
+
 def _vals8(vals):
     vals = np.asarray(vals)
     if vals.dtype.kind == "f":
@@ -162,12 +177,13 @@ def _vals8(vals):
 
 def map_task(keys, vals, P, op="sum", thresholds=None, combine=True):
     """ShuffleMapTask._run (dpark/task.py:209-226) over one input split.
-    Returns (bucket_keys:int64, bucket_vals, bucket_offsets[P+1]) bucket-major,
+    Returns (bucket_keys, bucket_vals, bucket_offsets[P+1]) bucket-major,
     each bucket in first-seen order.  combine=False keeps every row (the layout
-    the CUDA partition kernel produces before any combine)."""
+    the CUDA partition kernel produces before any combine).  Integer keys come back
+    as int64, float keys in their own dtype."""
     keys = np.ascontiguousarray(keys)
     h = hash_vec(keys)
-    k64 = keys.astype(np.int64) if keys.dtype != np.int64 else keys
+    k64 = _key_bits(keys)
     v8, vk = _vals8(vals)
     n = len(k64)
     ok = np.empty(n, dtype=np.int64)
@@ -180,25 +196,27 @@ def map_task(keys, vals, P, op="sum", thresholds=None, combine=True):
         thr_p, nthr = _p(thr), len(thr)
     tot = lib().orc_map_task(_p(k64), _p(h), _p(v8), vk, n, P, thr_p, nthr, OPS[op],
                              1 if combine else 0, _p(ok), _p(ov), _p(offs))
-    return ok[:tot], ov[:tot], offs
+    return _keys_from_bits(ok[:tot], keys.dtype), ov[:tot], offs
 
 
 def merge(keys, vals, op="sum"):
     """DiskHashMerger._merge (dpark/shuffle.py:600-608): distinct keys in
     first-seen order with combined values."""
-    k64 = np.ascontiguousarray(keys, dtype=np.int64)
+    keys = np.asarray(keys)
+    k64 = _key_bits(keys)
     v8, vk = _vals8(vals)
     n = len(k64)
     ok = np.empty(n, dtype=np.int64)
     ov = np.empty(n, dtype=v8.dtype)
     nd = lib().orc_merge(_p(k64), _p(v8), vk, n, OPS[op], _p(ok), _p(ov))
-    return ok[:nd], ov[:nd]
+    return _keys_from_bits(ok[:nd], keys.dtype), ov[:nd]
 
 
 def group(keys, vals):
     """OrderedGroupByDiskHashMerger (dpark/shuffle.py:626-646): CSR
     (keys, offsets, values); rows must arrive concatenated in map_id order."""
-    k64 = np.ascontiguousarray(keys, dtype=np.int64)
+    keys = np.asarray(keys)
+    k64 = _key_bits(keys)
     v = np.ascontiguousarray(vals)
     assert v.dtype.itemsize == 8
     n = len(k64)
@@ -206,7 +224,7 @@ def group(keys, vals):
     oo = np.empty(n + 1, dtype=np.int64)
     ov = np.empty(n, dtype=v.dtype)
     nd = lib().orc_group(_p(k64), _p(v.view(np.int64)), n, _p(ok), _p(oo), _p(ov.view(np.int64)))
-    return ok[:nd], oo[:nd + 1], ov
+    return _keys_from_bits(ok[:nd], keys.dtype), oo[:nd + 1], ov
 
 
 def reduce_by_key(key_splits, val_splits, P, op="sum", thresholds=None):

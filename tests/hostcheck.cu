@@ -49,4 +49,15 @@ int hc_bucket(const int64_t *h, int64_t n, int32_t P, int32_t sub_bits, int32_t 
     for (int64_t i = 0; i < n; i++) o[i] = f.bucket(h[i]);
     return 0;
 }
+int hc_choose_sb2(int64_t n, int32_t F, int32_t target_rows) { return dpk::choose_sb2(n, F, target_rows); }
+// the fine bucket of the reduce side's second-level split, numbered as dpk_combine does (first-level bucket * 2^sb2 +
+// fine): the first level as hc_bucket, the second by the mode 5 functor dpk_combine builds for the split
+int hc_fine_bucket(const int64_t *h, int64_t n, int32_t P, int32_t sub_bits, int32_t sb2, int32_t *o) {
+    dpk::PartFn f;
+    int rc = dpk::make_partfn(P, nullptr, 0, sub_bits, &f);
+    if (rc) return rc;
+    const dpk::PartFn fine = dpk::fine_partfn(f, sb2);
+    for (int64_t i = 0; i < n; i++) o[i] = (f.bucket(h[i]) << sb2) | fine.bucket(h[i]);
+    return 0;
+}
 }

@@ -4,6 +4,7 @@ import pytest
 import torch
 
 from oracle import oracle as orc
+from tests.shuffle_cases import dpk_options  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -308,7 +309,7 @@ def test_group_by_key_zipf_c3_shape_matches_oracle():
     assert hot > n // 20          # the skew is really there: the hottest key holds > 5 % of the rows
 
 
-def test_reduce_by_key_zipf_hot_keys_all_impls_sum_exact():
+def test_reduce_by_key_zipf_hot_keys_all_impls_sum_exact(dpk_options):
     """Skewed reduceByKey (hot key = ~10 % of the rows): shared-memory and global atomics pile up
     on one accumulator; sums stay exact."""
     from dpark_b200 import shuffle
@@ -317,11 +318,8 @@ def test_reduce_by_key_zipf_hot_keys_all_impls_sum_exact():
     v = np.random.default_rng(8).integers(-5, 6, n, dtype=np.int64)
     want = orc.reduce_by_key([k], [v], P, "sum")
     for impl in (2, 1):
-        nv().set_option("reduce_impl", impl)
-        try:
-            got = _parts_from(shuffle.reduce_by_key([dev(k)], [dev(v)], P, "sum"))
-        finally:
-            nv().set_option("reduce_impl", 2)
+        dpk_options({"reduce_impl": impl})
+        got = _parts_from(shuffle.reduce_by_key([dev(k)], [dev(v)], P, "sum"))
         for p in range(P):
             o1, o2 = np.argsort(got[p][0]), np.argsort(want[p][0])
             assert np.array_equal(got[p][0][o1], want[p][0][o2])

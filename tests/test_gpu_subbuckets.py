@@ -1,11 +1,15 @@
 """Sub-bucketed layout (sub_bits > 0): an internal refinement of each reduce
 partition.  What the reference defines must be unchanged: which keys a partition
 owns, and the (map split, position) order of rows -- now per fine bucket.  -m gpu."""
+import functools
+
 import numpy as np
 import pytest
 import torch
 
 from oracle import oracle as orc
+from tests.shuffle_cases import (COPY_VARIANTS, DEFAULT_OPTIONS, POINTER_VARIANTS, REDUCE_SHAPES,  # noqa: F401
+                                 REDUCE_VARIANTS, dpk_options, reduce_shape, variant_id)
 
 pytestmark = pytest.mark.gpu
 
@@ -71,39 +75,39 @@ def test_reduce_by_key_same_result_for_any_sub_bits(sb, op):
         assert np.array_equal(gv[o1], want[p][1][o2])
 
 
-@pytest.mark.parametrize("impl", [0, 1, 2])
-@pytest.mark.parametrize("shape", ["distinct_overflow", "hot_keys", "sentinel_key"])
-def test_every_reduce_implementation_gives_the_oracle_result(impl, shape):
-    """The three reduce-side implementations (dpk_set_option reduce_impl) must agree with
-    the oracle, including the cases that stress implementation 2: fine buckets with more
-    distinct keys than the shared-memory table holds (hash-disjoint passes), a few very hot
-    keys, and the key whose bits equal the free-slot marker (INT64_MIN)."""
+@functools.lru_cache(maxsize=None)
+def _shape_with_oracle(shape):
+    inputs, P, sb = reduce_shape(shape)
+    return [(k, v, orc.reduce_by_key([k], [v], P, "sum")) for k, v in inputs], P, sb
+
+
+def _reduce_variant_id(opts):
+    """The default and the reduce_impl variants keep the ids of the implementations they are ("2", "1", "0")."""
+    if not opts:
+        return str(DEFAULT_OPTIONS["reduce_impl"])
+    return str(opts["reduce_impl"]) if list(opts) == ["reduce_impl"] else variant_id(opts)
+
+
+@pytest.mark.parametrize("variant", REDUCE_VARIANTS, ids=_reduce_variant_id)
+@pytest.mark.parametrize("shape", REDUCE_SHAPES)
+def test_every_reduce_implementation_gives_the_oracle_result(variant, shape, dpk_options):
+    """Every reduce-side variant (the implementations of dpk_set_option reduce_impl, the merge kernels and launch
+    forms of implementation 2, the second-level split's target) must give the oracle's (int64, sum) result on the
+    shapes of tests/shuffle_cases.reduce_shape: mostly distinct keys (one window per fine bucket), a few very hot keys
+    (fine buckets of many windows), more distinct keys per fine bucket than a table holds (hash-disjoint passes), the
+    key whose bits equal the free-slot marker (INT64_MIN), and inputs of 0, 1 and 31 rows over 64 partitions.
+    tests/test_host_logic.py checks that each shape reaches the path it is named for."""
     from dpark_b200 import shuffle
-    rng = np.random.default_rng(77)
-    P, sb = 2, 0
-    if shape == "distinct_overflow":
-        n = 3_000_000                       # 1 first-level bucket per partition -> ~5.8 k rows per fine bucket
-        k = rng.permutation(n).astype(np.int64) * 7919 - 10 ** 9
-    elif shape == "hot_keys":
-        n = 1_000_000
-        k = rng.integers(0, 5, n, dtype=np.int64)
-        k[::7] = rng.integers(0, 10 ** 6, len(k[::7]))
-    else:
-        n = 200_000
-        k = rng.integers(-100, 100, n, dtype=np.int64)
-        k[::3] = -2 ** 63
-    v = rng.integers(-1000, 1000, n, dtype=np.int64)
-    nv().set_option("reduce_impl", impl)
-    try:
+    inputs, P, sb = _shape_with_oracle(shape)
+    dpk_options(variant)
+    for k, v, want in inputs:
         res = shuffle.reduce_by_key([dev(k)], [dev(v)], P, "sum", sub_bits=sb)
-    finally:
-        nv().set_option("reduce_impl", 2)
-    want = orc.reduce_by_key([k], [v], P, "sum")
-    for p, gk, gv in res:
-        gk, gv = gk.cpu().numpy(), gv.cpu().numpy()
-        o1, o2 = np.argsort(gk), np.argsort(want[p][0])
-        assert np.array_equal(gk[o1], want[p][0][o2])
-        assert np.array_equal(gv[o1], want[p][1][o2])
+        assert [p for p, _, _ in res] == list(range(P))
+        for p, gk, gv in res:
+            gk, gv = gk.cpu().numpy(), gv.cpu().numpy()
+            o1, o2 = np.argsort(gk), np.argsort(want[p][0])
+            assert np.array_equal(gk[o1], want[p][0][o2])
+            assert np.array_equal(gv[o1], want[p][1][o2])
 
 
 def test_reduce_with_thresholds_and_sub_buckets():
@@ -154,11 +158,13 @@ def test_pointer_mode_scatter_equals_plain_scatter():
     assert torch.equal(ok, mo.keys) and torch.equal(ov, mo.vals) and torch.equal(off, mo.offsets)
 
 
-@pytest.mark.parametrize("threads", [512, 1024])
+@pytest.mark.parametrize("variant", POINTER_VARIANTS,
+                         ids=lambda o: str(o["scatter_ptr_threads"]) if list(o) == ["scatter_ptr_threads"] else variant_id(o))
 @pytest.mark.parametrize("kinds", [("int64", "int64"), ("int32", "float32"), ("int64", None)])
-def test_pointer_mode_bulk_scatter_unordered(kinds, threads):
+def test_pointer_mode_bulk_scatter_unordered(kinds, variant, dpk_options):
     """The fused scatter + exchange for unordered multisplits (reduceByKey map side): k_part_scatter_bulk in pointer
-    mode -- bucket runs leave through the TMA to per-bucket absolute addresses.  With local addresses of buckets laid
+    mode -- bucket runs leave through the TMA to per-bucket absolute addresses (scatter_ptr_bulk 0: the round-1
+    kernel's pointer mode instead).  With local addresses of buckets laid
     out in a PERMUTED order (as in a peer's receive buffer, where a bucket's slot has nothing to do with its number)
     every bucket must hold exactly the rows the plain multisplit puts there, as a multiset of (key, value) pairs."""
     rng = np.random.default_rng(7)
@@ -168,26 +174,23 @@ def test_pointer_mode_bulk_scatter_unordered(kinds, threads):
     k = rng.integers(-2 ** 30, 2 ** 30, n).astype(kdt)
     v = None if vdt is None else (np.arange(n).astype(vdt))
     dk, dv = dev(k), (None if v is None else dev(v))
-    nv().set_option("scatter_ptr_threads", threads)
-    try:
-        pk, pv, off = nv().partition(dk, dv, P, sub_bits=sb, unordered=True)
-        counts, ws = nv().partition_count(dk, P, sub_bits=sb, unordered=True)
-        assert torch.equal(counts, off[1:] - off[:-1])
-        perm = torch.from_numpy(rng.permutation(F)).cuda()
-        # bucket b's slot: buckets laid out in perm order, 3 pad rows between slots (odd alignment phases)
-        c_perm = counts[perm]
-        start_perm = torch.cumsum(c_perm + 3, 0) - (c_perm + 3)
-        start = torch.empty(F, dtype=torch.int64, device="cuda")
-        start[perm] = start_perm
-        total = int((c_perm + 3).sum().item())
-        ok = torch.zeros(total, dtype=dk.dtype, device="cuda")
-        ov = None if dv is None else torch.zeros(total, dtype=dv.dtype, device="cuda")
-        kp = (ok.data_ptr() + start * ok.element_size()).contiguous()
-        vp = None if dv is None else (ov.data_ptr() + start * ov.element_size()).contiguous()
-        nv().partition_scatter_ptrs(dk, dv, P, kp, vp, ws, sub_bits=sb, unordered=True)
-        torch.cuda.synchronize()
-    finally:
-        nv().set_option("scatter_ptr_threads", 1024)
+    dpk_options(variant)
+    pk, pv, off = nv().partition(dk, dv, P, sub_bits=sb, unordered=True)
+    counts, ws = nv().partition_count(dk, P, sub_bits=sb, unordered=True)
+    assert torch.equal(counts, off[1:] - off[:-1])
+    perm = torch.from_numpy(rng.permutation(F)).cuda()
+    # bucket b's slot: buckets laid out in perm order, 3 pad rows between slots (odd alignment phases)
+    c_perm = counts[perm]
+    start_perm = torch.cumsum(c_perm + 3, 0) - (c_perm + 3)
+    start = torch.empty(F, dtype=torch.int64, device="cuda")
+    start[perm] = start_perm
+    total = int((c_perm + 3).sum().item())
+    ok = torch.zeros(total, dtype=dk.dtype, device="cuda")
+    ov = None if dv is None else torch.zeros(total, dtype=dv.dtype, device="cuda")
+    kp = (ok.data_ptr() + start * ok.element_size()).contiguous()
+    vp = None if dv is None else (ov.data_ptr() + start * ov.element_size()).contiguous()
+    nv().partition_scatter_ptrs(dk, dv, P, kp, vp, ws, sub_bits=sb, unordered=True)
+    torch.cuda.synchronize()
     okh, pkh = ok.cpu().numpy(), pk.cpu().numpy()
     ovh, pvh = (None, None) if dv is None else (ov.cpu().numpy(), pv.cpu().numpy())
     offh, sth, ch = off.cpu().numpy(), start.cpu().numpy(), counts.cpu().numpy()
@@ -345,8 +348,8 @@ def test_pipe_plan_layout(H, Q, kdt, vdt):
                 assert np.array_equal(seg[q], counts[:, lo:lo + part_blk])
 
 
-@pytest.mark.parametrize("tma", [0, 1])
-def test_copy_segments_on_a_few_sms(tma):
+@pytest.mark.parametrize("tma", [opts["copy_tma"] for opts in COPY_VARIANTS])
+def test_copy_segments_on_a_few_sms(tma, dpk_options):
     """dpk_copy_segments restricted to whole SMs (the overlapped pushes): the TMA ring (congruent segments: head / aligned
     middle / tail; incongruent ones by loads and stores) and the load/store form must both copy exactly the bytes of
     every segment and nothing else."""
@@ -367,12 +370,9 @@ def test_copy_segments_on_a_few_sms(tma):
         want[d_off:d_off + n] = srch[s_off:s_off + n]
         s_at = s_off + n + 40
         d_at = d_off + n + 40
-    nv().set_option("copy_tma", tma)
-    try:
-        nv().copy_segments(dev(np.array(so, dtype=np.int64)), dev(np.array(do, dtype=np.int64)), dev(np.array(nb, dtype=np.int64)), sms=3)
-        torch.cuda.synchronize()
-    finally:
-        nv().set_option("copy_tma", 1)
+    dpk_options({"copy_tma": tma})
+    nv().copy_segments(dev(np.array(so, dtype=np.int64)), dev(np.array(do, dtype=np.int64)), dev(np.array(nb, dtype=np.int64)), sms=3)
+    torch.cuda.synchronize()
     assert np.array_equal(dst.cpu().numpy(), want)
 
 
@@ -389,7 +389,7 @@ def test_choose_sub_bits_bounds():
 @pytest.mark.parametrize("wide", [0, 1])
 @pytest.mark.parametrize("op", ["sum", "min", "max"])
 @pytest.mark.parametrize("vkind", ["i64", "f64"])
-def test_slot_claim_variants_agree_with_the_oracle(wide, op, vkind):
+def test_slot_claim_variants_agree_with_the_oracle(wide, op, vkind, dpk_options):
     """dpk_set_option("agg_wide"): claiming a shared-memory slot and depositing the first value with one
     128-bit CAS (1) or with a 64-bit key CAS followed by an atomic on the accumulator (0) must both give
     the reference's createCombiner/mergeValue result (dpark/rdd.py:303-327) for every op and value kind,
@@ -403,11 +403,8 @@ def test_slot_claim_variants_agree_with_the_oracle(wide, op, vkind):
         v = rng.integers(-2 ** 40, 2 ** 40, n, dtype=np.int64)
     else:
         v = rng.standard_normal(n) * 1e6
-    nv().set_option("agg_wide", wide)
-    try:
-        res = shuffle.reduce_by_key([dev(k[: n // 2]), dev(k[n // 2:])], [dev(v[: n // 2]), dev(v[n // 2:])], P, op)
-    finally:
-        nv().set_option("agg_wide", 1)
+    dpk_options({"agg_wide": wide})
+    res = shuffle.reduce_by_key([dev(k[: n // 2]), dev(k[n // 2:])], [dev(v[: n // 2]), dev(v[n // 2:])], P, op)
     want = orc.reduce_by_key([k[: n // 2], k[n // 2:]], [v[: n // 2], v[n // 2:]], P, op)
     for p, gk, gv in res:
         gk, gv = gk.cpu().numpy(), gv.cpu().numpy()

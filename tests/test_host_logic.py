@@ -420,3 +420,92 @@ def test_merge_part_results_concatenates_partitions_in_order():
     assert po.tolist() == [0, 5, 7, 9, 11] and cnt.tolist() == [3, 1, 1, 2]
     got = [(k[po[j]:po[j] + cnt[j]].tolist(), v[po[j]:po[j] + cnt[j]].tolist()) for j in range(4)]
     assert got == [([10, 11, 12], [1, 2, 3]), ([20], [4]), ([30], [5]), ([40, 41], [6, 7])]
+
+
+# ------------------------------------------- oracle float keys, path coverage of the parity shapes
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+def test_oracle_keys_float_columns_by_value(dtype):
+    """orc.reduce_by_key / group_by_key key float columns by their canonical bits: 1.25 and 1.75 stay two keys,
+    -0.0 and 0.0 are one (spelled 0.0), infinities, subnormals and 2.0**61 (whose hash equals that of 1.0) are keys
+    of their own -- as in the reference's dicts (orc.py_reduce_by_key)."""
+    rng = np.random.default_rng(11)
+    pool = np.array([1.25, 1.75, -1.25, 0.0, -0.0, np.inf, -np.inf, 5e-324, -5e-324, 1e-310, 2.0 ** 61, 1.0, 3.0,
+                     2.0 ** -149, 1e-40, -7.5], dtype=np.float64).astype(dtype)
+    k = pool[rng.integers(0, len(pool), 600)]
+    v = rng.integers(-1000, 1000, len(k), dtype=np.int64)
+    ks, vs = np.array_split(k, 3), np.array_split(v, 3)
+    P = 3
+    want = orc.py_reduce_by_key([list(zip((float(x) for x in a), (int(y) for y in b))) for a, b in zip(ks, vs)],
+                                P, operator.add)
+    got = orc.reduce_by_key(ks, vs, P, "sum")
+    groups = orc.group_by_key(ks, [np.arange(len(a), dtype=np.int64) + 1000 * s for s, a in enumerate(ks)], P)
+    for p in range(P):
+        gk, gv = got[p]
+        assert gk.dtype == dtype
+        assert not np.signbit(gk[gk == 0]).any()
+        assert dict(zip((float(x) for x in gk), gv.tolist())) == want[p]
+        assert len(gk) == len(want[p])
+        wk, wo, _ = groups[p]
+        assert wk.dtype == dtype and sorted(float(x) for x in wk) == sorted(want[p])
+        assert [int(n) for n in np.diff(wo)] == [sum(float(x) == float(key) for x in k
+                                                     if orc.get_partition(float(x), P) == p) for key in wk]
+
+
+def test_every_set_option_switch_is_in_a_variant_table():
+    """Every switch dpk_set_option accepts has its default in tests/shuffle_cases.DEFAULT_OPTIONS, and every one
+    that selects a kernel variant is run against the oracle by a variant table (agg_timing only prints, copy_sms is
+    a parameter of copy_segments)."""
+    from tests import shuffle_cases as sc
+    src = open(os.path.join(ROOT, "dpark_b200", "csrc", "dpk_combine.cu")).read()
+    accepted = set(re.findall(r'strcmp\(name, "(\w+)"\)', src))
+    assert accepted == set(sc.DEFAULT_OPTIONS)
+    header = open(os.path.join(ROOT, "include", "dpark_b200.h")).read()
+    assert all('"%s"' % name in header for name in accepted)
+    tables = sc.REDUCE_VARIANTS + sc.MULTISPLIT_VARIANTS + sc.POINTER_VARIANTS + sc.COPY_VARIANTS
+    run = {name for opts in tables for name in opts}
+    assert accepted - {"agg_timing", "copy_sms"} <= run
+
+
+def _fine_buckets(L, keys, P, sb, n_total):
+    """Fine bucket of every key as dpk_combine's second-level split numbers it, for a combine over n_total rows."""
+    sb = 0 if sb is None else sb
+    sb2 = L.hc_choose_sb2(C.c_int64(n_total), C.c_int32(P << sb), C.c_int32(2048))
+    h = orc.hash_vec(keys)
+    fb = np.empty(len(h), dtype=np.int32)
+    assert L.hc_fine_bucket(_p(h), C.c_int64(len(h)), C.c_int32(P), C.c_int32(sb), C.c_int32(sb2), _p(fb)) == 0
+    return fb, sb2
+
+
+def test_reduce_parity_shapes_reach_their_kernel_paths():
+    """The reduce-side parity shapes (tests/shuffle_cases.reduce_shape) really hold what they are named for under the
+    current split tuning: `distinct_overflow` has a fine bucket with more than 2 x 2048 distinct keys (>= 4
+    hash-disjoint passes of k_smem_aggregate2, >= 2 of the round-1 kernel with its 3584-key limit), `hot_keys` a fine
+    bucket of more than one 2048-row window with few distinct keys, and `distinct` fits one window everywhere."""
+    from tests import shuffle_cases as sc
+    from dpark_b200 import shuffle
+    L = _hostcheck()
+    L.hc_choose_sb2.restype = C.c_int
+    for target in (64, 2048, 3584):
+        assert L.hc_choose_sb2(C.c_int64(6_000_000), C.c_int32(1), C.c_int32(target)) == 10    # capped at 1024-way
+    assert L.hc_choose_sb2(C.c_int64(2048), C.c_int32(1), C.c_int32(2048)) == 0
+    assert L.hc_choose_sb2(C.c_int64(4096), C.c_int32(1), C.c_int32(2048)) == 1
+    assert L.hc_choose_sb2(C.c_int64(4096 * 2), C.c_int32(2), C.c_int32(2048)) == 1
+
+    [(k, _)], P, sb = sc.reduce_shape("distinct_overflow")
+    fb, sb2 = _fine_buckets(L, k, P, sb, len(k))
+    distinct = np.bincount(fb, minlength=(P << sb) << sb2)          # every key is distinct
+    assert len(np.unique(k)) == len(k)
+    assert distinct.max() > 2 * sc.AG2_CAP and distinct.max() > sc.AG_LIMIT
+
+    [(k, _)], P, sb = sc.reduce_shape("hot_keys")
+    fb, sb2 = _fine_buckets(L, k, P, sb, len(k))
+    rows = np.bincount(fb)
+    pairs = np.unique(np.stack([fb.astype(np.int64), k]), axis=1)
+    nd = np.bincount(pairs[0], minlength=len(rows))
+    big = rows > sc.AG2_CAP
+    assert big.any() and nd[big].max() < sc.AG2_CAP // 4
+
+    [(k, _)], P, sb = sc.reduce_shape("distinct")
+    sb = shuffle.choose_sub_bits(len(k), P)
+    fb, sb2 = _fine_buckets(L, k, P, sb, len(k))
+    assert np.bincount(fb).max() <= sc.AG2_CAP
