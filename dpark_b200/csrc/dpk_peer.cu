@@ -214,7 +214,8 @@ k_copy_segments_tma(const uint64_t *__restrict__ src_ptrs, const uint64_t *__res
 //                      rank's receive buffer, element size
 // Outputs: src_ptrs / dst_ptrs / nbytes [ncols][G] (clamped so that nothing is written past `capacity` rows of the
 // region), need_over = max(need_over, max_d rows d receives - capacity), seg_out[S][blk_hi - blk_lo clipped to F]
-// (the segment matrix of my own part).
+// (the segment matrix of my own part: the rows that land in my region, so that a reduce over an overflowed step never
+// reads or sizes anything past `capacity` rows; that step's result is invalid and need_over says so).
 __global__ void __launch_bounds__(256)
 k_push_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_t F, int32_t per_blk, int32_t blk_lo,
             int32_t blk_hi, int64_t dst_row0, int32_t my_src, int32_t my_rank, int32_t ncols, uint64_t src0, uint64_t src1,
@@ -259,10 +260,18 @@ k_push_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_
         }
         if (total > capacity) atomicMax(need_over, total - capacity);
     }
-    if (seg_out) {
+    if (seg_out) {   // the rows that LAND here: source s's push is clamped at `capacity` rows of the region
         const int b0 = min(F, my_rank * per_blk + blk_lo), b1 = min(F, min((my_rank + 1) * per_blk, my_rank * per_blk + blk_hi));
         const int fo = b1 - b0;
-        for (int i = threadIdx.x; i < S * fo; i += blockDim.x) seg_out[i] = all_counts[(int64_t)(i / fo) * F + b0 + i % fo];
+        for (int s = threadIdx.x; s < S; s += blockDim.x) {
+            long long at = 0;                                  // row of source s's first row in my region
+            for (int t = 0; t < s; t++) at += s_R[t * G + my_rank];
+            for (int j = 0; j < fo; j++) {
+                const long long c = all_counts[(int64_t)s * F + b0 + j];
+                seg_out[(int64_t)s * fo + j] = max(0LL, min(c, capacity - at));
+                at += c;
+            }
+        }
     }
 }
 
@@ -276,7 +285,8 @@ k_push_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_
 //   all_counts[S][F], per_blk, my_src, my_rank: as in k_push_plan;  part_blk = buckets per part (per_blk / Q);
 //   region = rows of one part's region in a receive buffer (part q starts at row q * region)
 // Outputs: bucket_base[F] (row of bucket b's first row in the send buffer), src_ptrs / dst_ptrs / nbytes [Q][ncols][G],
-// need_over, seg_out[Q][S][part_blk] (own part columns; clipped columns hold 0) if not NULL.  Single CTA.
+// need_over, seg_out[Q][S][part_blk] (own part columns, the rows that land in region q; clipped columns hold 0) if not
+// NULL.  Single CTA.
 __global__ void __launch_bounds__(256)
 k_pipe_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_t F, int32_t per_blk, int32_t Q,
             int32_t part_blk, int64_t region, int32_t align_rows, int32_t my_src, int32_t my_rank, int32_t ncols,
@@ -334,11 +344,17 @@ k_pipe_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_
             run += s_mine[b];
         }
     }
-    if (seg_out) {
-        for (int i = threadIdx.x; i < Q * S * part_blk; i += blockDim.x) {
-            const int q = i / (S * part_blk), s = (i / part_blk) % S, j = i % part_blk;
-            const int b = my_rank * per_blk + q * part_blk + j;
-            seg_out[i] = (b < F && b < (my_rank + 1) * per_blk) ? all_counts[(int64_t)s * F + b] : 0;
+    if (seg_out) {   // the rows that LAND here: every push into region q is clamped at `region` rows
+        for (int i = threadIdx.x; i < Q * S; i += blockDim.x) {
+            const int q = i / S, s = i % S;
+            long long at = 0;                                  // row of source s's first row in region q
+            for (int t = 0; t < s; t++) at += s_R[((int64_t)q * S + t) * G + my_rank];
+            for (int j = 0; j < part_blk; j++) {
+                const int b = my_rank * per_blk + q * part_blk + j;
+                const long long c = (b < F && b < (my_rank + 1) * per_blk) ? all_counts[(int64_t)s * F + b] : 0;
+                seg_out[(int64_t)i * part_blk + j] = max(0LL, min(c, region - at));
+                at += c;
+            }
         }
     }
 }
@@ -348,7 +364,8 @@ k_pipe_plan(const int64_t *__restrict__ all_counts, int32_t S, int32_t G, int32_
 // source-rank-major then bucket-major exactly as the push form delivers it -- plus this rank's segment matrix and the
 // capacity flag.  A bucket that would end past `capacity` rows of its receive buffer is pointed at a local dump buffer
 // instead (dump0/dump1: >= this rank's row count; position = the bucket's local bucket-major offset), so a too-small
-// buffer can never be overrun; need_over reports it.  Single CTA; G <= 64 ranks, F <= 4096 buckets.
+// buffer can never be overrun; need_over reports it, and the segment matrix counts such a bucket as 0 rows (it
+// describes what landed).  Single CTA; G <= 64 ranks, F <= 4096 buckets.
 __global__ void __launch_bounds__(256)
 k_fused_plan(const int64_t *__restrict__ all_counts, int32_t G, int32_t F, int32_t per_blk, int32_t my_rank, int32_t ncols,
              const uint64_t *__restrict__ dst_base, int32_t elem0, int32_t elem1, int64_t capacity, uint64_t dump0,
@@ -387,9 +404,17 @@ k_fused_plan(const int64_t *__restrict__ all_counts, int32_t G, int32_t F, int32
         }
         if (total > capacity) atomicMax(need_over, total - capacity);
     }
-    if (seg_out) {
+    if (seg_out) {   // the rows that LAND here: a bucket diverted to its source's dump counts 0
         const int b0 = min(F, my_rank * per_blk), b1 = min(F, (my_rank + 1) * per_blk), fo = b1 - b0;
-        for (int i = threadIdx.x; i < G * fo; i += blockDim.x) seg_out[i] = all_counts[(int64_t)(i / fo) * F + b0 + i % fo];
+        for (int s = threadIdx.x; s < G; s += blockDim.x) {
+            long long at = 0;                                  // row of source s's first row in my buffer
+            for (int t = 0; t < s; t++) at += s_R[t * G + my_rank];
+            for (int j = 0; j < fo; j++) {
+                const long long c = all_counts[(int64_t)s * F + b0 + j];
+                seg_out[(int64_t)s * fo + j] = at + c <= capacity ? c : 0;
+                at += c;
+            }
+        }
     }
 }
 

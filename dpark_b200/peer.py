@@ -153,6 +153,15 @@ def push_plan(all_counts, blocks, rank):
     return edge[rank, :-1].contiguous(), src_base[rank].contiguous(), R[rank].contiguous(), R.sum(0)
 
 
+def _landed(seg, capacity):
+    """The segment matrix of the rows that land in a receive buffer of `capacity` rows (source-major, bucket-major;
+    every push is clamped at the capacity), as dpk_push_plan writes it: a reduce over an overflowed step must not read
+    or size anything past the buffer."""
+    flat = seg.reshape(-1)
+    start = torch.cumsum(flat, 0) - flat
+    return torch.minimum(flat, (capacity - start).clamp(min=0)).view(seg.shape).contiguous()
+
+
 def exchange_push(px, mo, need_host_count=False):
     """shuffle.exchange() over peer memory: the bucket-major map output `mo` stays local, and ONE
     launch of dpk_copy_segments pushes each peer's contiguous block (keys and values) into that
@@ -269,7 +278,8 @@ def shuffle_pipelined(px, key_chunks, val_chunks, P, op, thresholds=None, sub_bi
 
     Needs map splits that are consecutive slices of one buffer per group and nparts divisible into `parts` (else fewer
     parts are used).  Returns [(keys, vals, part_offsets, counts, part_first, nparts)] -- one reduce_side result per
-    part, in partition order."""
+    part, in partition order; a rank that owns no partitions gets one empty part (nparts 0), so that every rank's list
+    merges (merge_part_results) into a well-typed result."""
     from . import shuffle as sh
     G, rank, dev = px.world, px.rank, px.device
     F = P << sub_bits
@@ -403,15 +413,22 @@ def shuffle_pipelined(px, key_chunks, val_chunks, P, op, thresholds=None, sub_bi
         rv = None if vals is None else vals[q * region:(q + 1) * region]
         ok, ov, po, cnt = nv.combine(rk, rv, op, P, seg, first + p0, p1 - p0, thresholds, sub_bits)
         results.append((ok, ov, po, cnt, first + p0, p1 - p0))
+    if not results:   # a rank that owns no partitions (rank * ceil(P / G) >= P): one empty part, typed like the others
+        z = torch.zeros(1, dtype=torch.int64, device=dev)
+        ev = None if vals is None else torch.empty(0, dtype=nv.acc_dtype(vals.dtype), device=dev)
+        results.append((keys[:0], ev, z, z[:0], first, 0))
     px.advance()
     return results
 
 
 def merge_part_results(results):
     """One (keys, vals, part_offsets, counts) like shuffle.reduce_side from shuffle_pipelined's per-part results
-    (copies; for checks and callers that want one buffer -- the pipelined step itself never needs it)."""
+    (copies; for checks and callers that want one buffer -- the pipelined step itself never needs it).  Raises
+    NativeError if a part's merge failed (out_counts -1), as every other reduce-side consumer does."""
+    from .shuffle import check_counts
     ks, vs, pos, cnts, base = [], [], [], [], 0
     for ok, ov, po, cnt, _, _ in results:
+        check_counts(cnt.cpu().tolist())
         n = int(po[-1].item())
         ks.append(ok[:n])
         vs.append(ov[:n])
@@ -487,7 +504,7 @@ def _map_exchange_overlapped_splits(px, key_chunks, val_chunks, P, thresholds=No
                     t.record_stream(px.side)
     main.wait_stream(px.side)
     px.barrier()                                                        # every peer's stores have landed
-    seg = all_counts[:, b0:b1].contiguous()
+    seg = _landed(all_counts[:, b0:b1], px.capacity)
     keys, vals = px.keys, (px.vals if has_v else None)
     px.advance()
     return Received(keys, vals, seg, b0 >> sub_bits, (b1 - b0) >> sub_bits, sub_bits, bound=True)

@@ -101,17 +101,19 @@ class MapOutput(object):
 
 
 def _as_one(chunks):
-    """One tensor spanning `chunks` if they are consecutive contiguous slices of the same storage, else None."""
+    """One tensor spanning `chunks` if they are consecutive contiguous slices of the same storage, else None.
+    Positions are storage offsets: an empty slice's data_ptr() is not its place in the buffer, and a map split may be
+    empty."""
     first = chunks[0]
     if first is None or not first.is_contiguous():
         return None
     base = first.untyped_storage().data_ptr()
-    ptr, total = first.data_ptr(), 0
+    at, total = first.storage_offset(), 0
     for c in chunks:
-        if (c is None or c.dtype != first.dtype or c.dim() != 1 or not c.is_contiguous() or c.data_ptr() != ptr
+        if (c is None or c.dtype != first.dtype or c.dim() != 1 or not c.is_contiguous() or c.storage_offset() != at
                 or c.untyped_storage().data_ptr() != base):
             return None
-        ptr += c.numel() * c.element_size()
+        at += c.numel()
         total += c.numel()
     return torch.empty(0, dtype=first.dtype, device=first.device).set_(first.untyped_storage(), first.storage_offset(), (total,))
 

@@ -157,7 +157,9 @@ int dpk_memcpy_batch(const uint64_t *h_dst_ptrs, const uint64_t *h_src_ptrs, con
  * src_keys / src_vals (ncols = 1: keys only), rank d's receive buffer for column c at dst_base[c * nranks + d] (device
  * array), elements are key_bytes / val_bytes wide.  Writes src_ptrs / dst_ptrs /
  * nbytes [ncols][nranks] (pushes are clamped to `capacity` rows per receive buffer), *need_over = max(*need_over,
- * rows the fullest receive buffer lacks) and, if seg_out != NULL, seg_out[nsrc][own buckets] for dpk_combine. */
+ * rows the fullest receive buffer lacks) and, if seg_out != NULL, seg_out[nsrc][own buckets] for dpk_combine: the rows
+ * that land in my buffer, so after a clamped push it describes no row past `capacity` (the step's result is invalid,
+ * need_over reports it, but the reduce side stays inside its buffers). */
 int dpk_push_plan(const int64_t *all_counts, int32_t nsrc, int32_t nranks, int32_t nbuckets, int32_t per_block,
                   int32_t my_src, int32_t my_rank, int32_t ncols, uint64_t src_keys, uint64_t src_vals,
                   const uint64_t *dst_base, int32_t key_bytes, int32_t val_bytes, int64_t capacity, uint64_t *src_ptrs,
@@ -178,7 +180,8 @@ int dpk_push_plan_part(const int64_t *all_counts, int32_t nsrc, int32_t nranks, 
  * front of every (destination, part) block the send buffer holds up to 16 / min(key_bytes, val_bytes) - 1 pad rows so
  * that source and destination of every push are congruent mod 16 bytes (the copy then runs through the TMA); size it
  * rows + nranks * nparts * (16 / min element size).  seg_out[nparts][nsrc][per_block / nparts]: the segment matrices of
- * my own parts for dpk_combine (columns beyond my last bucket are 0).  need_over as in dpk_push_plan, per region. */
+ * my own parts for dpk_combine (the rows that land in each region; columns beyond my last bucket are 0).  need_over as
+ * in dpk_push_plan, per region. */
 int dpk_pipe_plan(const int64_t *all_counts, int32_t nsrc, int32_t nranks, int32_t nbuckets, int32_t per_block,
                   int32_t nparts, int64_t region_rows, int32_t my_src, int32_t my_rank, int32_t ncols, uint64_t src_keys,
                   uint64_t src_vals, const uint64_t *dst_base, int32_t key_bytes, int32_t val_bytes, int64_t *bucket_base,
@@ -189,7 +192,8 @@ int dpk_pipe_plan(const int64_t *all_counts, int32_t nsrc, int32_t nranks, int32
  * laid out source-rank-major then bucket-major exactly as the push delivers it.  A bucket that would end past
  * `capacity` rows of the owner's buffer is pointed into the local dump columns dump_keys / dump_vals (>= this rank's
  * row count) at its local bucket-major offset, and *need_over reports the overflow, so a too-small receive buffer is
- * never overrun.  nbuckets <= 4096.  Replaces, with dpk_partition_scatter_ptrs, the reducers' pull of every map
+ * never overrun; seg_out[nranks][own buckets] (if not NULL) counts the rows that land, 0 for a diverted bucket.
+ * nbuckets <= 4096.  Replaces, with dpk_partition_scatter_ptrs, the reducers' pull of every map
  * output over files + HTTP (dpark/shuffle.py:309-420) by stores over NVLink issued by the map-side scatter itself. */
 int dpk_fused_plan(const int64_t *all_counts, int32_t nranks, int32_t nbuckets, int32_t per_block, int32_t my_rank,
                    int32_t ncols, const uint64_t *dst_base, int32_t key_bytes, int32_t val_bytes, int64_t capacity,

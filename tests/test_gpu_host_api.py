@@ -129,10 +129,10 @@ def test_map_side_combine_gives_the_same_partitions(op):
 
 
 @pytest.mark.parametrize("G,P,sb,H", [(2, 8, 0, 1), (3, 5, 1, 1), (8, 64, 3, 1), (4, 1, 3, 1), (8, 5, 2, 2)])
-def test_push_plan_kernel_equals_the_tensor_plan(G, P, sb, H):
+def test_push_plan_kernel_equals_the_tensor_plan_with_landed_segments(G, P, sb, H):
     """dpk_push_plan (one launch) against peer.push_plan (the tensor arithmetic the CPU tests pin to the alltoallv
     layout): segment table of every source row, clamping at the receive-buffer capacity, the capacity flag and the
-    segment matrix of the rank's own buckets."""
+    segment matrix of the rows that land in the rank's own buckets."""
     from dpark_b200 import _native as nv
     from dpark_b200 import peer, shuffle
     rng = np.random.default_rng(G * 100 + P)
@@ -156,4 +156,7 @@ def test_push_plan_kernel_equals_the_tensor_plan(G, P, sb, H):
                 assert torch.equal(dst[:G], dst_base[:G] + df * 8) and torch.equal(dst[G:], dst_base[G:] + df * 4)
                 assert torch.equal(nby[:G], rows * 8) and torch.equal(nby[G:], rows * 4)
                 assert int(need) == max(0, int(tot.max()) - cap)
-                assert torch.equal(seg, counts[:, blocks[rank]:blocks[rank + 1]])
+                # the segment matrix describes the rows that land: every source's push is clamped at the capacity
+                mine = counts[:, blocks[rank]:blocks[rank + 1]]
+                assert torch.equal(seg, peer._landed(mine, cap))
+                assert int(seg.sum()) == min(int(mine.sum()), cap)
