@@ -35,7 +35,7 @@ EXPORTS = [
     "dpk_key_or", "dpk_radix_pass", "dpk_group_heads_workspace_bytes", "dpk_group_heads", "dpk_gather_i64",
     "dpk_partition_scatter_ptrs", "dpk_copy_segments", "dpk_hash_tuple", "dpk_push_plan", "dpk_push_plan_part", "dpk_pipe_plan", "dpk_fused_plan", "dpk_memcpy_batch",
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
-    "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg",
+    "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
 ]
 
 _lib = None
@@ -97,6 +97,9 @@ def lib():
         L.dpk_dict_encode_workspace_bytes.restype = i64
         L.dpk_dict_encode_workspace_bytes.argtypes = [i64]
         L.dpk_dict_encode.argtypes = [vp, vp, vp, i64, vp, vp, i64, vp]
+        L.dpk_join_count.argtypes = [vp, vp, i64, i64, i32, i32, vp, vp, vp]
+        L.dpk_join_emit.argtypes = [vp, vp, vp, vp, vp, i64, i64, vp, i32, vp, i32, i32, i32, i64, vp, vp, vp, vp, vp,
+                                    vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -540,6 +543,34 @@ def group_heads(sorted_keys):
     _check(lib().dpk_group_heads(_ptr(sorted_keys), n, _ptr(out_keys), _ptr(out_starts), _ptr(ng), _ptr(ws),
                                  ws_bytes, _stream()))
     return out_keys, out_starts, ng
+
+
+# ---- f1: join expansion -----------------------------------------------------------
+def join_count(ids, group_starts, G, nL, keep_left, keep_right):
+    """Per group of the tagged union's CSR: (nl[G], out_count[G]) int64 device tensors (dpk_join_count)."""
+    _need_cuda(ids, group_starts)
+    nl = torch.empty(G, dtype=torch.int64, device=ids.device)
+    cnt = torch.empty(G, dtype=torch.int64, device=ids.device)
+    _check(lib().dpk_join_count(_ptr(ids), _ptr(group_starts), G, nL, int(keep_left), int(keep_right), _ptr(nl),
+                                _ptr(cnt), _stream()))
+    return nl, cnt
+
+
+def join_emit(group_keys, group_starts, ids, nl, out_off, nL, lvals, rvals, keep_left, keep_right, n_out):
+    """The joined rows (dpk_join_emit): (keys int64, left, right, left_valid uint8 | None, right_valid uint8 | None);
+    values keep their dtypes, a valid column exists only for a side the join kind can miss."""
+    _need_cuda(group_keys, group_starts, ids, nl, out_off, lvals, rvals)
+    dev = ids.device
+    keys = torch.empty(n_out, dtype=torch.int64, device=dev)
+    left = torch.empty(n_out, dtype=lvals.dtype, device=dev)
+    right = torch.empty(n_out, dtype=rvals.dtype, device=dev)
+    lvalid = torch.empty(n_out, dtype=torch.uint8, device=dev) if keep_right else None
+    rvalid = torch.empty(n_out, dtype=torch.uint8, device=dev) if keep_left else None
+    _check(lib().dpk_join_emit(_ptr(group_keys), _ptr(group_starts), _ptr(ids), _ptr(nl), _ptr(out_off),
+                               int(nl.numel()), nL, _ptr(lvals), lvals.element_size(), _ptr(rvals), rvals.element_size(),
+                               int(keep_left), int(keep_right), n_out, _ptr(keys), _ptr(left), _ptr(right),
+                               _ptr(lvalid), _ptr(rvalid), _stream()))
+    return keys, left, right, lvalid, rvalid
 
 
 def set_option(name, value):

@@ -264,6 +264,31 @@ DPK_HD PartFn fine_partfn(const PartFn &first, int sb2) {
     return fine;
 }
 
+// ------------------------------------------------------------- f1: join arithmetic (dpk_join.cu; tests/joincheck.cu
+// runs the same functions on the CPU)
+// A group's id run ids[0 .. len) holds its left rows (ids < nL) before its right rows: the map side is a stable
+// multisplit, the radix passes are stable and the left splits come first.  So the left count is a binary search.
+DPK_HD int64_t join_left_rows(const int64_t *run, int64_t len, int64_t nL) {
+    int64_t lo = 0, hi = len;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (run[mid] < nL) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+// rows a side contributes to the cross product: its own rows, or one None row when it has none and the OTHER side's
+// unmatched keys are kept (dpark_b200/rdd.py _join: `if not left and keep_right: left = [None]`)
+DPK_HD int64_t join_side(int64_t n, bool keep_other) { return n > 0 ? n : (keep_other ? 1 : 0); }
+DPK_HD int64_t join_count(int64_t nl, int64_t nr, bool keep_left, bool keep_right) {
+    return join_side(nl, keep_right) * join_side(nr, keep_left);
+}
+// output row i of a group -> (a, b): left row a, right row b, `for a in left for b in right`
+DPK_HD void join_pair(int64_t i, int64_t nr, bool keep_left, int64_t *a, int64_t *b) {
+    const int64_t R = join_side(nr, keep_left);
+    *a = i / R;
+    *b = i - *a * R;
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

@@ -42,6 +42,20 @@ def _emit(res, P, part_off, gkeys, gstarts, ids, objs, key_decoder):
     return res
 
 
+def group_row_ids(key_chunks, id_chunks, P, thresholds):
+    """The numeric group-by on one GPU: map_side -> exchange -> group_side over int64 / float64 device key columns
+    (the map splits in order) carrying int64 row ids.  Returns (group_keys[G] as int64 bits, group_starts[G + 1],
+    ids, part_offsets[P + 1]): group g holds ids[group_starts[g] : group_starts[g + 1]] in (map split, position)
+    order, groups are partition-major.  One host read (G)."""
+    float_keys = key_chunks[0].dtype == torch.float64
+    mo = shuffle.map_side(key_chunks, id_chunks, P, thresholds)
+    rx = shuffle.exchange(mo)
+    rx.keys = rx.keys.view(torch.int64)
+    gk, gs, ng, ov, off = shuffle.group_side(rx, P, thresholds, key_view=torch.float64 if float_keys else None)
+    G = int(ng.item())
+    return gk[:G], gs[:G + 1], ov, off
+
+
 def group_by_key(splits, P, thresholds, dev, res):
     if shuffle._world() > 1:
         raise NotImplementedError("this is the one-GPU stage; under torch.distributed the rows are first routed to the "
@@ -62,16 +76,11 @@ def group_by_key(splits, P, thresholds, dev, res):
         kc = [torch.from_numpy(c.keys.astype(kdt, copy=False)).to(dev) for c in splits]
         vc = [torch.arange(int(bounds[i]), int(bounds[i + 1]), dtype=torch.int64, device=dev)
               for i in range(len(splits))]
-        mo = shuffle.map_side(kc, vc, P, thresholds)
-        rx = shuffle.exchange(mo)
-        view = None if kk == columnar.KEY_I64 else torch.float64
-        rx.keys = rx.keys.view(torch.int64)
-        gk, gs, ng, ov, off = shuffle.group_side(rx, P, thresholds, key_view=view)
-        G = int(ng.item())
-        gkeys = gk[:G].cpu().numpy()
+        gk, gs, ov, off = group_row_ids(kc, vc, P, thresholds)
+        gkeys = gk.cpu().numpy()
         if kk == columnar.KEY_F64:
             gkeys = gkeys.view(np.float64)
-        return _emit(res, P, off.cpu().numpy(), gkeys, gs[:G + 1].cpu().numpy(), ov.cpu().numpy(), objs,
+        return _emit(res, P, off.cpu().numpy(), gkeys, gs.cpu().numpy(), ov.cpu().numpy(), objs,
                      lambda a: a.tolist())
     # ---- str / bytes keys
     data = np.concatenate([c.keys for c in splits if c.n]) if n else np.zeros(0, np.uint8)

@@ -1,0 +1,113 @@
+"""join / leftOuterJoin / rightOuterJoin / outerJoin of two numeric ColumnarRDDs on one GPU (dpark/rdd.py:649-676).
+
+RDD._join is a cogroup followed by a flatMap over Python lists: every row of the inputs and of the result becomes a
+Python object.  When both inputs already are columns the same result is computed on the device:
+
+  1. the left keys, then the right keys, converted as columnar._key_column converts Python keys (int32 -> int64,
+     float32 -> float64, + 0.0), go through the numeric group-by (grouping.group_row_ids) carrying their row ids, so
+     row id < nL is a left row; the values stay where they are, in the same concatenated order;
+  2. dpk_join_count: per key its left row count and the L * R rows it produces;
+  3. the exclusive scan of those counts places every key's rows; the partitions' row offsets are read back once;
+  4. dpk_join_emit: the joined rows, load-balanced over output rows, the values gathered by row id.
+
+The groups come out partition by partition in the order of the group-by of the tagged union, and per key
+`for x in left for y in right` -- partitions, rows and order are those of the composition.
+"""
+import torch
+
+from . import _native as nv
+from . import grouping, spmd
+from .rdd import RDD, ColumnarRDD, Split
+
+DTYPES = (torch.int32, torch.int64, torch.float32, torch.float64)
+
+
+def device_join_applies(a, b):
+    """True when a join of a and b runs on the device: two ColumnarRDDs (not subclasses), one process, 1-D key and
+    value columns of int32 / int64 / float32 / float64."""
+    if type(a) is not ColumnarRDD or type(b) is not ColumnarRDD:
+        return False
+    if spmd.rank_world()[1] != 1:
+        return False
+    return all(t.dtype in DTYPES and t.dim() == 1 for t in (a.keys, a.vals, b.keys, b.vals))
+
+
+def _key_column(left, right, dev):
+    """The left keys followed by the right keys on the device, as the row path ingests them; raises TypeError where
+    it does (NaN keys, int keys on one side and float keys on the other)."""
+    sides = [k for k in (left.keys, right.keys) if k.numel()]
+    for k in sides:
+        if k.dtype.is_floating_point and bool(torch.isnan(k).any()):
+            raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
+    kinds = sorted(set("float" if k.dtype.is_floating_point else "int" for k in sides))
+    if len(kinds) > 1:
+        raise TypeError("mixed key types %s in one shuffle are not supported on the GPU path" % kinds)
+    kdt = torch.float64 if kinds == ["float"] else torch.int64
+    keys = torch.cat([left.keys.to(dev, kdt), right.keys.to(dev, kdt)])
+    return keys + 0.0 if kdt == torch.float64 else keys     # -0.0 and 0.0 are one key, spelled 0.0
+
+
+def join_columns(left, right, P, thresholds, keep_left, keep_right):
+    """The joined rows of two ColumnarRDDs: a list of P tuples (keys, left, right, left_valid, right_valid) of CUDA
+    tensors, one per partition."""
+    from .engine import _device
+    dev = _device()
+    nL = int(left.keys.numel())
+    keys = _key_column(left, right, dev)
+    lvals, rvals = left.vals.to(dev).contiguous(), right.vals.to(dev).contiguous()
+    n = int(keys.numel())
+    if n == 0:
+        out = (keys, lvals, rvals, torch.empty(0, dtype=torch.uint8, device=dev) if keep_right else None,
+               torch.empty(0, dtype=torch.uint8, device=dev) if keep_left else None)
+        return [out] * P
+    ids = torch.arange(n, dtype=torch.int64, device=dev)
+    gk, gs, ov, part_off = grouping.group_row_ids([keys], [ids], P, thresholds)
+    G = int(gk.numel())
+    nl, cnt = nv.join_count(ov, gs, G, nL, keep_left, keep_right)
+    out_off = torch.zeros(G + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(cnt, 0, out=out_off[1:])
+    # partition p's rows start at the output offset of its first group; the last entry is the total
+    bounds = out_off[torch.searchsorted(gs[:-1], part_off)].cpu().tolist()
+    cols = nv.join_emit(gk, gs, ov, nl, out_off, nL, lvals, rvals, keep_left, keep_right, bounds[-1])
+    if keys.dtype == torch.float64:
+        cols = (cols[0].view(torch.float64),) + cols[1:]
+    return [tuple(None if c is None else c[bounds[p]:bounds[p + 1]] for c in cols) for p in range(P)]
+
+
+class ColumnarJoinedRDD(RDD):
+    """The result of join / leftOuterJoin / rightOuterJoin / outerJoin of two numeric ColumnarRDDs in a one-process
+    job: the rows RDD._join's composition yields, computed on the GPU the first time a partition is asked for and
+    kept (like ShuffledRDD).  Like the flatMap it stands for, it has the cogroup's partitions and no partitioner."""
+
+    def __init__(self, left, right, part, keep_left, keep_right):
+        RDD.__init__(self, left.ctx)
+        self.left, self.right = left, right
+        self.join_partitioner = part
+        self.keep_left, self.keep_right = keep_left, keep_right
+        self._splits = [Split(i) for i in range(part.numPartitions)]
+        self._result = None
+
+    def parents(self):
+        return [self.left, self.right]
+
+    def _materialize(self):
+        if self._result is None:
+            p = self.join_partitioner
+            self._result = join_columns(self.left, self.right, p.numPartitions, p.thresholds, self.keep_left,
+                                        self.keep_right)
+        return self._result
+
+    def columns(self, split):
+        """Extension: partition `split` as CUDA tensors (keys, left, right, left_valid, right_valid).  Keys are int64
+        or float64, values keep their input dtypes; a valid column is uint8 (0 = the side is missing, its value slot
+        holds 0) and None for a side the join kind never misses."""
+        return self._materialize()[split.index]
+
+    def compute(self, split):
+        keys, left, right, lvalid, rvalid = self.columns(split)
+        ls, rs = left.cpu().tolist(), right.cpu().tolist()
+        if lvalid is not None:
+            ls = [x if ok else None for x, ok in zip(ls, lvalid.cpu().tolist())]
+        if rvalid is not None:
+            rs = [y if ok else None for y, ok in zip(rs, rvalid.cpu().tolist())]
+        return zip(keys.cpu().tolist(), zip(ls, rs))

@@ -239,12 +239,19 @@ class RDD(object):
         if isinstance(others, RDD):
             others = [others]
         others = list(others)
+        return CoGroupedRDD([self] + others, self._cogroup_partitioner(others, numSplits, fixSkew), taskMemory,
+                            rddconf=rddconf)
+
+    def _cogroup_partitioner(self, others, numSplits, fixSkew):
+        """The partitioner of a cogroup of self and others (dpark/rdd.py:686-731): numSplits defaults to self's
+        partition count if self is partitioned, else defaultParallelism; fixSkew > 0 samples hash thresholds over
+        the union of the inputs."""
         if numSplits is None:
             numSplits = self.partitioner.numPartitions if self.partitioner is not None else self.ctx.defaultParallelism
         thresh = None
         if fixSkew > 0 and numSplits > 1:
             thresh, numSplits = self.union(*others)._skew_thresholds(numSplits, fixSkew)
-        return CoGroupedRDD([self] + others, HashPartitioner(numSplits, thresholds=thresh), taskMemory, rddconf=rddconf)
+        return HashPartitioner(numSplits, thresholds=thresh)
 
     cogroup = groupWith
 
@@ -263,8 +270,15 @@ class RDD(object):
 
     def _join(self, other, keeps, numSplits=None, taskMemory=None, fixSkew=-1, rddconf=None):
         """dpark/rdd.py:661-676: the cross product of the two value lists of every key; `keeps` names the sides
-        (1 = left, 2 = right) whose unmatched keys survive, paired with None."""
+        (1 = left, 2 = right) whose unmatched keys survive, paired with None.
+
+        Two numeric ColumnarRDDs in a one-process job are joined on the device (dpark_b200/join.py), with the same
+        partitions, rows and order as this composition."""
         keep_left, keep_right = 1 in keeps, 2 in keeps
+        from . import join
+        if join.device_join_applies(self, other):
+            return join.ColumnarJoinedRDD(self, other, self._cogroup_partitioner([other], numSplits, fixSkew),
+                                          keep_left, keep_right)
 
         def pairs(row):
             k, (left, right) = row

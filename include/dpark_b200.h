@@ -298,6 +298,27 @@ int64_t dpk_group_heads_workspace_bytes(int64_t n);
 int dpk_group_heads(const int64_t *sorted_keys, int64_t n, int64_t *out_keys, int64_t *out_starts,
                     int64_t *out_ngroups, void *ws, int64_t ws_bytes, dpk_stream_t stream);
 
+/* ---- f1: join / leftOuterJoin / rightOuterJoin / outerJoin (dpark/rdd.py:649-676) over columns --------------------
+ * Input: the CSR of a groupByKey of the tagged union (dpk_group_heads over the sorted rows): group g's row ids are
+ * ids[group_starts[g] .. group_starts[g+1]), where ids < nL are left rows (left value nr. id) and the others right
+ * rows (right value nr. id - nL).  Left ids precede right ids inside every group (the group-by is stable and the
+ * left rows come first).  keep_left / keep_right: unmatched keys of that side survive, paired with a missing value.
+ *   dpk_join_count : out_nl[g] = left rows of group g; out_count[g] = L * R, L = nl ? nl : keep_right,
+ *                    R = nr ? nr : keep_left (int64, ngroups entries each).
+ *   dpk_join_emit  : out_off[ngroups + 1] = the exclusive scan of out_count (n_out = out_off[ngroups]).  Output row
+ *                    out_off[g] + a * R + b of group g: out_keys = group_keys[g] (int64 bits), out_left = left value
+ *                    a, out_right = right value b, in the order `for a in left for b in right`.  A missing side
+ *                    writes value 0 and valid flag 0; out_lvalid (uint8) is written iff keep_right, out_rvalid iff
+ *                    keep_left, and must then be given.  lval_bytes / rval_bytes in {4, 8}, chosen independently; lvals / rvals
+ *                    may be NULL when that side has no rows. */
+int dpk_join_count(const int64_t *ids, const int64_t *group_starts, int64_t ngroups, int64_t nL, int32_t keep_left,
+                   int32_t keep_right, int64_t *out_nl, int64_t *out_count, dpk_stream_t stream);
+int dpk_join_emit(const int64_t *group_keys, const int64_t *group_starts, const int64_t *ids, const int64_t *nl,
+                  const int64_t *out_off, int64_t ngroups, int64_t nL, const void *lvals, int32_t lval_bytes,
+                  const void *rvals, int32_t rval_bytes, int32_t keep_left, int32_t keep_right, int64_t n_out,
+                  int64_t *out_keys, void *out_left, void *out_right, uint8_t *out_lvalid, uint8_t *out_rvalid,
+                  dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
