@@ -36,6 +36,7 @@ EXPORTS = [
     "dpk_partition_scatter_ptrs", "dpk_copy_segments", "dpk_hash_tuple", "dpk_push_plan", "dpk_push_plan_part", "dpk_pipe_plan", "dpk_fused_plan", "dpk_memcpy_batch",
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
+    "dpk_cogroup_count", "dpk_cogroup_emit",
 ]
 
 _lib = None
@@ -100,6 +101,8 @@ def lib():
         L.dpk_join_count.argtypes = [vp, vp, i64, i64, i32, i32, vp, vp, vp]
         L.dpk_join_emit.argtypes = [vp, vp, vp, vp, vp, i64, i64, vp, i32, vp, i32, i32, i32, i64, vp, vp, vp, vp, vp,
                                     vp]
+        L.dpk_cogroup_count.argtypes = [vp, vp, i64, vp, i32, vp, vp, vp]
+        L.dpk_cogroup_emit.argtypes = [vp, vp, vp, i64, i64, vp, i32, i64, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -571,6 +574,28 @@ def join_emit(group_keys, group_starts, ids, nl, out_off, nL, lvals, rvals, keep
                                int(keep_left), int(keep_right), n_out, _ptr(keys), _ptr(left), _ptr(right),
                                _ptr(lvalid), _ptr(rvalid), _stream()))
     return keys, left, right, lvalid, rvalid
+
+
+def cogroup_count(ids, group_starts, G, bounds):
+    """Per input t and group g of the cogroup's CSR (input t owns the ids [bounds[t], bounds[t + 1])): (first, count),
+    int64 device tensors [N, G] -- where input t's sub-run of group g starts in ids, and its length (dpk_cogroup_count)."""
+    _need_cuda(ids, group_starts, bounds)
+    N = int(bounds.numel()) - 1
+    first = torch.empty((N, G), dtype=torch.int64, device=ids.device)
+    cnt = torch.empty((N, G), dtype=torch.int64, device=ids.device)
+    _check(lib().dpk_cogroup_count(_ptr(ids), _ptr(group_starts), G, _ptr(bounds), N, _ptr(first), _ptr(cnt),
+                                   _stream()))
+    return first, cnt
+
+
+def cogroup_emit(ids, first, out_off, id_base, vals, n_out):
+    """One input's values, per group in its sub-run order (dpk_cogroup_emit): first[G] and out_off[G + 1] are that
+    input's rows of cogroup_count's first and of the exclusive scan of its counts; the values keep their dtype."""
+    _need_cuda(ids, first, out_off, vals)
+    out = torch.empty(n_out, dtype=vals.dtype, device=ids.device)
+    _check(lib().dpk_cogroup_emit(_ptr(ids), _ptr(first), _ptr(out_off), int(first.numel()), id_base, _ptr(vals),
+                                  vals.element_size(), n_out, _ptr(out), _stream()))
+    return out
 
 
 def set_option(name, value):

@@ -267,7 +267,8 @@ DPK_HD PartFn fine_partfn(const PartFn &first, int sb2) {
 // ------------------------------------------------------------- f1: join arithmetic (dpk_join.cu; tests/joincheck.cu
 // runs the same functions on the CPU)
 // A group's id run ids[0 .. len) holds its left rows (ids < nL) before its right rows: the map side is a stable
-// multisplit, the radix passes are stable and the left splits come first.  So the left count is a binary search.
+// multisplit, the radix passes are stable and the left splits come first.  So the left count is a binary search (the
+// lower bound of nL: the ids below it).
 DPK_HD int64_t join_left_rows(const int64_t *run, int64_t len, int64_t nL) {
     int64_t lo = 0, hi = len;
     while (lo < hi) {
@@ -287,6 +288,37 @@ DPK_HD void join_pair(int64_t i, int64_t nr, bool keep_left, int64_t *a, int64_t
     const int64_t R = join_side(nr, keep_left);
     *a = i / R;
     *b = i - *a * R;
+}
+// the last group g in [lo, hi) with off[g] <= i (off[lo] <= i holds): the group of output row i given the exclusive
+// scan off of the groups' row counts.  Empty groups share their offset with the next group, so the answer always has
+// rows.  The load-balanced emits of the join and the cogroup map their rows to groups with it.
+DPK_HD int64_t group_of(const int64_t *off, int64_t lo, int64_t hi, int64_t i) {
+    while (hi - lo > 1) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (off[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// ------------------------------------------------------------- f1: cogroup arithmetic (dpk_join.cu; tests/cogroupcheck.cu
+// runs the same functions on the CPU)
+// Input t of a cogroup owns the row ids [bounds[t], bounds[t + 1]).  A group's id run ids[s .. s + len) is ascending in
+// input order, so input t's sub-run starts where the ids below bounds[t] end: one lower-bound search per boundary.
+// Writes first[t * stride] (absolute position in ids) and count[t * stride] for t < ninputs.
+DPK_HD void cogroup_split(const int64_t *ids, int64_t s, int64_t len, const int64_t *bounds, int32_t ninputs,
+                          int64_t *first, int64_t *count, int64_t stride) {
+    int64_t lo = join_left_rows(ids + s, len, bounds[0]);
+    for (int32_t t = 0; t < ninputs; t++) {
+        const int64_t hi = join_left_rows(ids + s, len, bounds[t + 1]);
+        first[t * stride] = s + lo;
+        count[t * stride] = hi - lo;
+        lo = hi;
+    }
+}
+// output row r of one input, in the group that starts at output row base and whose sub-run starts at ids[first]: the
+// input's own row number (its values column is indexed from 0, its ids from id_base)
+DPK_HD int64_t cogroup_source(const int64_t *ids, int64_t first, int64_t base, int64_t r, int64_t id_base) {
+    return ids[first + r - base] - id_base;
 }
 
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)

@@ -10,6 +10,14 @@
 //                  no output rows occupies no row of any tile.
 // Algorithmic bytes of the emit: per output row 8 (key) + LW + RW written (+1 per valid flag), 8 + 8 (the two ids)
 // + LW + RW read; the group-level reads (out_off, starts, nl, keys) are per tile, not per row.
+//
+// groupWith / cogroup of N inputs (dpark/rdd.py:686-731) over the same CSR, input t owning the ids [bounds[t],
+// bounds[t + 1]): no cross product, every key's run is split N ways.
+//   k_cogroup_count : one thread per group; per input the start of its sub-run (a lower-bound search for bounds[t])
+//                     and its length (cogroup_split, dpk_common.cuh).
+//   k_cogroup_emit  : one launch per input, load-balanced over that input's output rows with the tile of k_join_emit;
+//                     output row r of group g is value ids[first[g] + r - out_off[g]] - id_base.
+// Algorithmic bytes of a cogroup emit: per output row 8 (the id) + W read, W written.
 #include "dpk_common.cuh"
 
 namespace dpk {
@@ -33,14 +41,46 @@ k_join_count(const int64_t *__restrict__ ids, const int64_t *__restrict__ starts
     out_count[g] = join_count(nl, len - nl, keep_left, keep_right);
 }
 
-// the last group g in [lo, hi) with off[g] <= i (off[lo] <= i holds); empty groups share their offset with the next
-// group, so the answer always has rows
-__device__ __forceinline__ int64_t group_of(const int64_t *off, int64_t lo, int64_t hi, int64_t i) {
-    while (hi - lo > 1) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (off[mid] <= i) lo = mid; else hi = mid;
+// The rows of one CTA of a load-balanced emit: a tile of JN_TILE output rows [i0, i_last], and the groups they fall in,
+// g0 .. g0 + span - 1, found by binary search on the exclusive scan off[G + 1] of the groups' row counts.  A tile's
+// rows belong to at most JN_TILE groups with rows, but empty groups between them also lie in that range: the offsets
+// are staged in shared memory (s_off[JN_TILE + 1]) when they fit, searched in place otherwise.
+struct EmitTile {
+    const int64_t *off, *s_off;
+    int64_t i0, i_last, g0, span;
+    bool staged;
+
+    // the group of output row i and that group's first output row
+    __device__ __forceinline__ void locate(int64_t i, int64_t *g, int64_t *base) const {
+        if (staged) {
+            const int64_t j = group_of(s_off, 0, span, i);
+            *g = g0 + j;
+            *base = s_off[j];
+        } else {
+            *g = group_of(off, g0, g0 + span, i);
+            *base = off[*g];
+        }
     }
-    return lo;
+};
+
+__device__ __forceinline__ EmitTile emit_tile(const int64_t *off, int64_t G, int64_t n_out, int64_t *s_off,
+                                              int64_t *s_g) {
+    EmitTile t;
+    t.off = off;
+    t.s_off = s_off;
+    t.i0 = (int64_t)blockIdx.x * JN_TILE;
+    t.i_last = min(t.i0 + JN_TILE, n_out) - 1;
+    // the groups of the tile's first and last rows
+    if (threadIdx.x == 0) s_g[0] = group_of(off, 0, G, t.i0);
+    if (threadIdx.x == 32) s_g[1] = group_of(off, 0, G, t.i_last);
+    __syncthreads();
+    t.g0 = s_g[0];
+    t.span = s_g[1] - t.g0 + 1;
+    t.staged = t.span <= JN_TILE;
+    if (t.staged)
+        for (int64_t j = threadIdx.x; j <= t.span; j += JN_THREADS) s_off[j] = off[t.g0 + j];
+    __syncthreads();
+    return t;
 }
 
 template <int LW, int RW>
@@ -54,32 +94,13 @@ k_join_emit(const int64_t *__restrict__ gkeys, const int64_t *__restrict__ start
     typedef typename ValWord<RW>::T RT;
     __shared__ int64_t s_off[JN_TILE + 1];
     __shared__ int64_t s_g[2];
-    const int64_t i0 = (int64_t)blockIdx.x * JN_TILE;
-    const int64_t i_last = min(i0 + JN_TILE, n_out) - 1;
-    // the groups of the tile's first and last rows
-    if (threadIdx.x == 0) s_g[0] = group_of(out_off, 0, G, i0);
-    if (threadIdx.x == 32) s_g[1] = group_of(out_off, 0, G, i_last);
-    __syncthreads();
-    const int64_t g0 = s_g[0], span = s_g[1] - g0 + 1;
-    // a tile's rows belong to at most JN_TILE groups with rows, but empty groups between them also lie in
-    // [g0, g1]: the offsets are staged in shared memory when they fit, searched in place otherwise
-    const bool staged = span <= JN_TILE;
-    if (staged)
-        for (int64_t j = threadIdx.x; j <= span; j += JN_THREADS) s_off[j] = out_off[g0 + j];
-    __syncthreads();
+    const EmitTile tile = emit_tile(out_off, G, n_out, s_off, s_g);
 #pragma unroll 2
     for (int it = 0; it < JN_ITEMS; it++) {
-        const int64_t i = i0 + (int64_t)it * JN_THREADS + threadIdx.x;
-        if (i > i_last) break;
+        const int64_t i = tile.i0 + (int64_t)it * JN_THREADS + threadIdx.x;
+        if (i > tile.i_last) break;
         int64_t g, base;
-        if (staged) {
-            const int64_t j = group_of(s_off, 0, span, i);
-            g = g0 + j;
-            base = s_off[j];
-        } else {
-            g = group_of(out_off, g0, g0 + span, i);
-            base = out_off[g];
-        }
+        tile.locate(i, &g, &base);
         const int64_t s = starts[g], nl = nls[g], nr = starts[g + 1] - s - nl;
         int64_t a, b;
         join_pair(i - base, nr, keep_left, &a, &b);
@@ -98,6 +119,37 @@ k_join_emit(const int64_t *__restrict__ gkeys, const int64_t *__restrict__ start
 typedef void (*EmitFn)(const int64_t *, const int64_t *, const int64_t *, const int64_t *, const int64_t *, int64_t,
                        int64_t, const void *, const void *, bool, int64_t, int64_t *, void *, void *, uint8_t *,
                        uint8_t *);
+
+// cogroup of N inputs: the same CSR split N ways (cogroup_split, dpk_common.cuh); out_first / out_count are
+// input-major [ninputs][G]
+__global__ void __launch_bounds__(256)
+k_cogroup_count(const int64_t *__restrict__ ids, const int64_t *__restrict__ starts, int64_t G,
+                const int64_t *__restrict__ bounds, int32_t ninputs, int64_t *__restrict__ out_first,
+                int64_t *__restrict__ out_count) {
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    const int64_t s = starts[g];
+    cogroup_split(ids, s, starts[g + 1] - s, bounds, ninputs, out_first + g, out_count + g, G);
+}
+
+// one input's value runs, load-balanced over its output rows like k_join_emit
+template <int W>
+__global__ void __launch_bounds__(JN_THREADS)
+k_cogroup_emit(const int64_t *__restrict__ ids, const int64_t *__restrict__ first, const int64_t *__restrict__ out_off,
+               int64_t G, int64_t id_base, const void *__restrict__ vals, int64_t n_out, void *__restrict__ out_vals) {
+    typedef typename ValWord<W>::T T;
+    __shared__ int64_t s_off[JN_TILE + 1];
+    __shared__ int64_t s_g[2];
+    const EmitTile tile = emit_tile(out_off, G, n_out, s_off, s_g);
+#pragma unroll 2
+    for (int it = 0; it < JN_ITEMS; it++) {
+        const int64_t i = tile.i0 + (int64_t)it * JN_THREADS + threadIdx.x;
+        if (i > tile.i_last) break;
+        int64_t g, base;
+        tile.locate(i, &g, &base);
+        static_cast<T *>(out_vals)[i] = static_cast<const T *>(vals)[cogroup_source(ids, first[g], base, i, id_base)];
+    }
+}
 
 }  // namespace dpk
 
@@ -144,6 +196,39 @@ int dpk_join_emit(const int64_t *group_keys, const int64_t *group_starts, const 
     DPK_LAUNCH("join_emit", st, fn<<<(unsigned)blocks, JN_THREADS, 0, st>>>(
         group_keys, group_starts, ids, nl, out_off, ngroups, nL, lvals, rvals, keep_left != 0, n_out, out_keys,
         out_left, out_right, keep_right ? out_lvalid : nullptr, keep_left ? out_rvalid : nullptr));
+    return DPK_OK;
+}
+
+int dpk_cogroup_count(const int64_t *ids, const int64_t *group_starts, int64_t ngroups, const int64_t *bounds,
+                      int32_t ninputs, int64_t *out_first, int64_t *out_count, dpk_stream_t stream) {
+    if (ngroups < 0 || ninputs < 1)
+        return fail(DPK_ERR_INVALID, "ngroups=%lld ninputs=%d", (long long)ngroups, (int)ninputs);
+    if (ngroups == 0) return DPK_OK;
+    if (!ids || !group_starts || !bounds || !out_first || !out_count) return fail(DPK_ERR_INVALID, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t blocks = (ngroups + 255) / 256;
+    DPK_LAUNCH("cogroup_count", st, k_cogroup_count<<<(unsigned)blocks, 256, 0, st>>>(
+        ids, group_starts, ngroups, bounds, ninputs, out_first, out_count));
+    return DPK_OK;
+}
+
+int dpk_cogroup_emit(const int64_t *ids, const int64_t *first, const int64_t *out_off, int64_t ngroups, int64_t id_base,
+                     const void *vals, int32_t val_bytes, int64_t n_out, void *out_vals, dpk_stream_t stream) {
+    if (ngroups < 0 || id_base < 0 || n_out < 0)
+        return fail(DPK_ERR_INVALID, "ngroups=%lld id_base=%lld n_out=%lld", (long long)ngroups, (long long)id_base,
+                    (long long)n_out);
+    if (val_bytes != 4 && val_bytes != 8) return fail(DPK_ERR_UNSUPPORTED, "value width %d bytes (4 or 8)", val_bytes);
+    if (n_out == 0) return DPK_OK;
+    if (!ids || !first || !out_off || !vals || !out_vals) return fail(DPK_ERR_INVALID, "NULL pointer");
+    if (ngroups == 0) return fail(DPK_ERR_INVALID, "n_out=%lld rows from no group", (long long)n_out);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t blocks = (n_out + JN_TILE - 1) / JN_TILE;
+    if (val_bytes == 8)
+        DPK_LAUNCH("cogroup_emit", st, k_cogroup_emit<8><<<(unsigned)blocks, JN_THREADS, 0, st>>>(
+            ids, first, out_off, ngroups, id_base, vals, n_out, out_vals));
+    else
+        DPK_LAUNCH("cogroup_emit", st, k_cogroup_emit<4><<<(unsigned)blocks, JN_THREADS, 0, st>>>(
+            ids, first, out_off, ngroups, id_base, vals, n_out, out_vals));
     return DPK_OK;
 }
 

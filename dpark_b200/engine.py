@@ -71,8 +71,22 @@ def run_shuffle(srdd):
                 return res
         splits = _gather_parent(srdd, True)
         return _run_reduce(splits, P, thr, srdd.op, dev)
+    from . import join
+    if join.device_path_applies([srdd.parent]):
+        return _run_group_columns(srdd.parent, P, thr)
     splits = _gather_parent(srdd, False)
     return _run_group(splits, P, thr, dev)
+
+
+def _run_group_columns(parent, P, thr):
+    """groupByKey of a numeric ColumnarRDD: the one-input cogroup on the device (dpark_b200/join.py), handed out as
+    the host lists the row path gives."""
+    from . import join
+    res = ShuffleResult(P)
+    for p, (keys, offsets, (vals,)) in enumerate(join.cogroup_columns([parent], P, thr)):
+        off, vs = offsets[0].cpu().tolist(), vals.cpu().tolist()
+        res.parts[p] = (keys.cpu().tolist(), [vs[off[j]:off[j + 1]] for j in range(len(off) - 1)])
+    return res
 
 
 # ---------------------------------------------------------------------------------------------------------------------

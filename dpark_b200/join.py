@@ -1,4 +1,5 @@
-"""join / leftOuterJoin / rightOuterJoin / outerJoin of two numeric ColumnarRDDs on one GPU (dpark/rdd.py:649-676).
+"""join / leftOuterJoin / rightOuterJoin / outerJoin of two numeric ColumnarRDDs on one GPU (dpark/rdd.py:649-676), and
+groupWith / cogroup / groupByKey of numeric ColumnarRDDs.
 
 RDD._join is a cogroup followed by a flatMap over Python lists: every row of the inputs and of the result becomes a
 Python object.  When both inputs already are columns the same result is computed on the device:
@@ -12,6 +13,10 @@ Python object.  When both inputs already are columns the same result is computed
 
 The groups come out partition by partition in the order of the group-by of the tagged union, and per key
 `for x in left for y in right` -- partitions, rows and order are those of the composition.
+
+groupWith / cogroup of N numeric ColumnarRDDs (CoGroupedRDD, a group-by of the tagged union) and groupByKey of one
+(N = 1) take the same CSR without a cross product: dpk_cogroup_count splits every key's id run at the inputs' id
+boundaries, and dpk_cogroup_emit gathers each input's value runs, load-balanced like the join's emit.
 """
 import torch
 
@@ -22,20 +27,20 @@ from .rdd import RDD, ColumnarRDD, Split
 DTYPES = (torch.int32, torch.int64, torch.float32, torch.float64)
 
 
-def device_join_applies(a, b):
-    """True when a join of a and b runs on the device: two ColumnarRDDs (not subclasses), one process, 1-D key and
-    value columns of int32 / int64 / float32 / float64."""
-    if type(a) is not ColumnarRDD or type(b) is not ColumnarRDD:
+def device_path_applies(rdds):
+    """True when a join, cogroup or groupByKey of rdds runs on the device: every input a ColumnarRDD (not a subclass),
+    one process, 1-D key and value columns of int32 / int64 / float32 / float64."""
+    if any(type(r) is not ColumnarRDD for r in rdds):
         return False
     if spmd.rank_world()[1] != 1:
         return False
-    return all(t.dtype in DTYPES and t.dim() == 1 for t in (a.keys, a.vals, b.keys, b.vals))
+    return all(t.dtype in DTYPES and t.dim() == 1 for r in rdds for t in (r.keys, r.vals))
 
 
-def _key_column(left, right, dev):
-    """The left keys followed by the right keys on the device, as the row path ingests them; raises TypeError where
-    it does (NaN keys, int keys on one side and float keys on the other)."""
-    sides = [k for k in (left.keys, right.keys) if k.numel()]
+def _key_column(rdds, dev):
+    """The keys of rdds one after the other on the device, as the row path ingests them; raises TypeError where it
+    does (NaN keys, int keys on one input and float keys on another)."""
+    sides = [r.keys for r in rdds if r.keys.numel()]
     for k in sides:
         if k.dtype.is_floating_point and bool(torch.isnan(k).any()):
             raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
@@ -43,7 +48,7 @@ def _key_column(left, right, dev):
     if len(kinds) > 1:
         raise TypeError("mixed key types %s in one shuffle are not supported on the GPU path" % kinds)
     kdt = torch.float64 if kinds == ["float"] else torch.int64
-    keys = torch.cat([left.keys.to(dev, kdt), right.keys.to(dev, kdt)])
+    keys = torch.cat([r.keys.to(dev, kdt) for r in rdds])
     return keys + 0.0 if kdt == torch.float64 else keys     # -0.0 and 0.0 are one key, spelled 0.0
 
 
@@ -53,7 +58,7 @@ def join_columns(left, right, P, thresholds, keep_left, keep_right):
     from .engine import _device
     dev = _device()
     nL = int(left.keys.numel())
-    keys = _key_column(left, right, dev)
+    keys = _key_column([left, right], dev)
     lvals, rvals = left.vals.to(dev).contiguous(), right.vals.to(dev).contiguous()
     n = int(keys.numel())
     if n == 0:
@@ -111,3 +116,72 @@ class ColumnarJoinedRDD(RDD):
         if rvalid is not None:
             rs = [y if ok else None for y, ok in zip(rs, rvalid.cpu().tolist())]
         return zip(keys.cpu().tolist(), zip(ls, rs))
+
+
+def cogroup_columns(rdds, P, thresholds):
+    """The cogroup of N ColumnarRDDs: a list of P tuples (keys[G_p], offsets[N, G_p + 1], (values_0, ..., values_N-1))
+    of CUDA tensors, one per partition.  Keys are int64 or float64, keys[j]'s values from input t are
+    values_t[offsets[t, j] : offsets[t, j + 1]] in input t's dtype and (split, position) order; every offsets row
+    starts at 0."""
+    from .engine import _device
+    dev = _device()
+    N = len(rdds)
+    keys = _key_column(rdds, dev)
+    vals = tuple(r.vals.to(dev).contiguous() for r in rdds)
+    sizes = [int(r.keys.numel()) for r in rdds]
+    bounds = [0]
+    for m in sizes:
+        bounds.append(bounds[-1] + m)
+    n = bounds[-1]
+    if n == 0:
+        return [(keys, torch.zeros((N, 1), dtype=torch.int64, device=dev), vals)] * P
+    ids = torch.arange(n, dtype=torch.int64, device=dev)
+    gk, gs, ov, part_off = grouping.group_row_ids([keys], [ids], P, thresholds)
+    G = int(gk.numel())
+    first, cnt = nv.cogroup_count(ov, gs, G, torch.tensor(bounds, dtype=torch.int64, device=dev))
+    off = torch.zeros((N, G + 1), dtype=torch.int64, device=dev)
+    for t in range(N):      # one 1-D scan per input: torch scans a [N, G] tensor along dim 1 one row per CTA
+        torch.cumsum(cnt[t], 0, out=off[t, 1:])
+    # partition p holds the groups [pg[p], pg[p + 1]) and input t's values [rows[t][p], rows[t][p + 1])
+    pg = torch.searchsorted(gs[:-1], part_off)
+    rows = off[:, pg].cpu().tolist()
+    pg = pg.cpu().tolist()
+    cols = [nv.cogroup_emit(ov, first[t], off[t], bounds[t], vals[t], rows[t][-1]) for t in range(N)]
+    if keys.dtype == torch.float64:
+        gk = gk.view(torch.float64)
+    return [(gk[pg[p]:pg[p + 1]], off[:, pg[p]:pg[p + 1] + 1] - off[:, pg[p]:pg[p] + 1],
+             tuple(cols[t][rows[t][p]:rows[t][p + 1]] for t in range(N))) for p in range(P)]
+
+
+class ColumnarCoGroupedRDD(RDD):
+    """The result of groupWith / cogroup of numeric ColumnarRDDs in a one-process job: per key one value list per
+    input, the rows CoGroupedRDD yields, computed on the GPU the first time a partition is asked for and kept.  It has
+    the cogroup's partitioner, so mapValue keeps it and a later groupWith reads it as a narrow dependency."""
+
+    def __init__(self, rdds, part):
+        RDD.__init__(self, rdds[0].ctx)
+        self.rdds = list(rdds)
+        self.partitioner = part
+        self._splits = [Split(i) for i in range(part.numPartitions)]
+        self._result = None
+
+    def parents(self):
+        return list(self.rdds)
+
+    def _materialize(self):
+        if self._result is None:
+            p = self.partitioner
+            self._result = cogroup_columns(self.rdds, p.numPartitions, p.thresholds)
+        return self._result
+
+    def columns(self, split):
+        """Extension: partition `split` as CUDA tensors (keys, offsets, values): keys int64 or float64, offsets int64
+        [N, keys + 1], values a tuple of N columns in the inputs' dtypes (see cogroup_columns)."""
+        return self._materialize()[split.index]
+
+    def compute(self, split):
+        keys, offsets, values = self.columns(split)
+        off = offsets.cpu().tolist()
+        vals = [v.cpu().tolist() for v in values]
+        groups = zip(*[[vs[o[j]:o[j + 1]] for j in range(len(o) - 1)] for o, vs in zip(off, vals)])
+        return zip(keys.cpu().tolist(), groups)

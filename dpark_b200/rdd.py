@@ -235,12 +235,18 @@ class RDD(object):
         return self.combineByKey(GroupByAggregator(), numSplits, taskMemory, fixSkew=fixSkew, rddconf=rddconf)
 
     def groupWith(self, others, numSplits=None, taskMemory=None, fixSkew=-1, rddconf=None):
-        """dpark/rdd.py:686-731: (k, (values of self, values of others[0], ...)) for every key of any input."""
+        """dpark/rdd.py:686-731: (k, (values of self, values of others[0], ...)) for every key of any input.
+
+        Numeric ColumnarRDDs in a one-process job are grouped on the device (dpark_b200/join.py), with the same
+        partitions, keys and value lists as CoGroupedRDD."""
         if isinstance(others, RDD):
             others = [others]
         others = list(others)
-        return CoGroupedRDD([self] + others, self._cogroup_partitioner(others, numSplits, fixSkew), taskMemory,
-                            rddconf=rddconf)
+        part = self._cogroup_partitioner(others, numSplits, fixSkew)
+        from . import join
+        if join.device_path_applies([self] + others):
+            return join.ColumnarCoGroupedRDD([self] + others, part)
+        return CoGroupedRDD([self] + others, part, taskMemory, rddconf=rddconf)
 
     def _cogroup_partitioner(self, others, numSplits, fixSkew):
         """The partitioner of a cogroup of self and others (dpark/rdd.py:686-731): numSplits defaults to self's
@@ -276,7 +282,7 @@ class RDD(object):
         partitions, rows and order as this composition."""
         keep_left, keep_right = 1 in keeps, 2 in keeps
         from . import join
-        if join.device_join_applies(self, other):
+        if join.device_path_applies([self, other]):
             return join.ColumnarJoinedRDD(self, other, self._cogroup_partitioner([other], numSplits, fixSkew),
                                           keep_left, keep_right)
 

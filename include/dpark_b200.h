@@ -319,6 +319,20 @@ int dpk_join_emit(const int64_t *group_keys, const int64_t *group_starts, const 
                   int64_t *out_keys, void *out_left, void *out_right, uint8_t *out_lvalid, uint8_t *out_rvalid,
                   dpk_stream_t stream);
 
+/* ---- f1: groupWith / cogroup of N inputs (dpark/rdd.py:686-731) over columns ---------------------------------------
+ * Input: the same CSR as the join, the ids of input t being [bounds[t], bounds[t+1]) (bounds: device, ninputs + 1
+ * entries, ascending).  Inside every group the ids ascend, so input t's rows of the group are one sub-run.
+ *   dpk_cogroup_count : out_first[t * ngroups + g] = the position in ids where input t's sub-run of group g starts,
+ *                       out_count[t * ngroups + g] = its length (input-major, ninputs * ngroups entries each).
+ *   dpk_cogroup_emit  : one input (first = its row of out_first, id_base = its bounds[t]); out_off[ngroups + 1] = the
+ *                       exclusive scan of its counts (n_out = out_off[ngroups]).  Output row r of group g
+ *                       (out_off[g] <= r < out_off[g+1]) is vals[ids[first[g] + r - out_off[g]] - id_base]: per key
+ *                       the input's values in (map split, position) order.  val_bytes in {4, 8}. */
+int dpk_cogroup_count(const int64_t *ids, const int64_t *group_starts, int64_t ngroups, const int64_t *bounds,
+                      int32_t ninputs, int64_t *out_first, int64_t *out_count, dpk_stream_t stream);
+int dpk_cogroup_emit(const int64_t *ids, const int64_t *first, const int64_t *out_off, int64_t ngroups, int64_t id_base,
+                     const void *vals, int32_t val_bytes, int64_t n_out, void *out_vals, dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
