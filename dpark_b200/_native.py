@@ -218,6 +218,33 @@ def partition_workspace(nbuckets, device):
 
 
 K_UNORDERED = 0x100   # DPK_K_UNORDERED: rows of a bucket may come out in any order
+K_PACKED = 0x200      # DPK_K_PACKED: rows are (key, value) records of one [n, 2] buffer instead of two columns
+
+
+def packable(keys, vals, prehashed=False):
+    """Whether (keys, vals) rows can travel as packed records: values as wide as the keys, hashed keys."""
+    return vals is not None and not prehashed and keys.element_size() == vals.element_size()
+
+
+def packed_views(rows, key_dtype, val_dtype):
+    """The key and value columns of a packed [n, 2] row buffer, as strided views."""
+    return rows[:, 0], (rows if val_dtype == rows.dtype else rows.view(val_dtype))[:, 1]
+
+
+def packed_source(keys, vals):
+    """The [n, 2] row buffer that keys and vals are the column views of (packed_views), or None."""
+    if keys is None or vals is None or keys.dim() != 1 or vals.dim() != 1 or keys.numel() != vals.numel():
+        return None
+    es = keys.element_size()
+    if (vals.element_size() != es or keys.stride() != (2,) or vals.stride() != (2,)
+            or vals.data_ptr() != keys.data_ptr() + es or keys.untyped_storage().data_ptr() != vals.untyped_storage().data_ptr()):
+        return None
+    return keys.as_strided((keys.numel(), 2), (2, 1))
+
+
+def packed_rows(n, key_dtype, device):
+    """An [n, 2] buffer of packed rows (the record alignment is the allocator's)."""
+    return torch.empty((n, 2), dtype=key_dtype, device=device)
 
 
 def _kk(keys, prehashed, row_hash, unordered=False):
@@ -241,10 +268,14 @@ def partition_count(keys, P, thresholds=None, prehashed=False, sub_bits=0, ws=No
 
 def partition_scatter(keys, vals, P, bucket_base, out_keys, out_vals, ws, thresholds=None, prehashed=False,
                       sub_bits=0, row_hash=None, unordered=False):
+    """out_vals None with vals given: out_keys is a packed [n, 2] row buffer (packed_rows)."""
     _need_cuda(keys, vals, bucket_base, out_keys, out_vals, ws, row_hash)
     thr, nthr = _thr(thresholds, keys.device)
     vb = 0 if vals is None else vals.element_size()
-    _check(lib().dpk_partition_scatter(_ptr(keys), _kk(keys, prehashed, row_hash, unordered), _ptr(row_hash), _ptr(vals), vb,
+    kk = _kk(keys, prehashed, row_hash, unordered)
+    if vals is not None and out_vals is None:
+        kk |= K_PACKED
+    _check(lib().dpk_partition_scatter(_ptr(keys), kk, _ptr(row_hash), _ptr(vals), vb,
                                        keys.numel(), P,
                                        _ptr(thr), nthr, sub_bits, _ptr(bucket_base), _ptr(out_keys),
                                        _ptr(out_vals), _ptr(ws), ws.numel(), _stream()))
@@ -360,9 +391,11 @@ def fused_plan(all_counts, nranks, per_block, my_rank, dst_base, key_bytes, val_
     return kp, vp_, seg
 
 
-def partition(keys, vals, P, thresholds=None, prehashed=False, sub_bits=0, row_hash=None, unordered=False):
+def partition(keys, vals, P, thresholds=None, prehashed=False, sub_bits=0, row_hash=None, unordered=False,
+              packed=False):
     """Stable hash-partition of one chunk (ShuffleMapTask._run, dpark/task.py:209-226).
-    Returns (out_keys, out_vals, offsets[(P << sub_bits) + 1] int64 device)."""
+    Returns (out_keys, out_vals, offsets[(P << sub_bits) + 1] int64 device); packed=True (packable rows):
+    (rows[n, 2], None, offsets), the rows written as packed records."""
     _need_cuda(keys, vals, row_hash)
     if vals is not None and vals.numel() != keys.numel():
         from .errors import DparkUserFatalError
@@ -370,11 +403,18 @@ def partition(keys, vals, P, thresholds=None, prehashed=False, sub_bits=0, row_h
     F = P << sub_bits
     thr, nthr = _thr(thresholds, keys.device)
     ws = partition_workspace(F, keys.device)
-    out_keys = torch.empty_like(keys)
-    out_vals = None if vals is None else torch.empty_like(vals)
+    kk = _kk(keys, prehashed, row_hash, unordered)
+    if packed:
+        if not packable(keys, vals, prehashed):
+            raise TypeError("packed rows need hashed keys and values of the same width")
+        out_keys, out_vals = packed_rows(keys.numel(), keys.dtype, keys.device), None
+        kk |= K_PACKED
+    else:
+        out_keys = torch.empty_like(keys)
+        out_vals = None if vals is None else torch.empty_like(vals)
     offsets = torch.empty(F + 1, dtype=torch.int64, device=keys.device)
     vb = 0 if vals is None else vals.element_size()
-    _check(lib().dpk_partition(_ptr(keys), _kk(keys, prehashed, row_hash, unordered), _ptr(row_hash), _ptr(vals), vb,
+    _check(lib().dpk_partition(_ptr(keys), kk, _ptr(row_hash), _ptr(vals), vb,
                                keys.numel(), P,
                                _ptr(thr), nthr, sub_bits, _ptr(out_keys), _ptr(out_vals), _ptr(offsets),
                                _ptr(ws), ws.numel(), _stream()))
@@ -389,7 +429,7 @@ def acc_dtype(vals_dtype):
 
 
 def combine(keys, vals, op, P, seg_rows, part_first=0, nparts=None, thresholds=None, sub_bits=0,
-            row_hash=None):
+            row_hash=None, rows=None):
     """Reduce-side merge (DiskHashMerger._merge, dpark/shuffle.py:600-608) of the
     rows of partitions [part_first, part_first+nparts).  Rows are laid out
     source-major, bucket-major inside; seg_rows: device int64 [nsrc, nparts <<
@@ -397,8 +437,14 @@ def combine(keys, vals, op, P, seg_rows, part_first=0, nparts=None, thresholds=N
     out_vals, out_offsets[nparts+1], out_counts[nparts]); partition j's distinct
     keys are out[out_offsets[j] : out_offsets[j] + out_counts[j]].  With row_hash
     (the per-row portable_hash column) the keys are representative row ids from
-    dict_encode (DPK_K_ROWID)."""
-    _need_cuda(keys, vals, seg_rows, row_hash)
+    dict_encode (DPK_K_ROWID).  rows: the packed [n, 2] buffer keys and vals are the column views of (the kernels
+    then read one record per row).  Column views of a packed buffer (MapOutput.keys / .vals) are recognised as such
+    without it."""
+    _need_cuda(seg_rows, row_hash, rows)
+    if rows is None:
+        rows = packed_source(keys, vals)
+    if rows is None:
+        _need_cuda(keys, vals)
     if nparts is None:
         nparts = P
     n = keys.numel()
@@ -412,12 +458,18 @@ def combine(keys, vals, op, P, seg_rows, part_first=0, nparts=None, thresholds=N
     thr, nthr = _thr(thresholds, keys.device)
     ws_bytes = lib().dpk_combine_workspace_bytes(n, F, nsrc)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=keys.device)
-    out_keys = torch.empty_like(keys)
+    out_keys = torch.empty(n, dtype=keys.dtype, device=keys.device)
     out_vals = torch.empty(n, dtype=acc_dtype(vals.dtype), device=keys.device)
     out_offsets = torch.empty(nparts + 1, dtype=torch.int64, device=keys.device)
     out_counts = torch.empty(nparts, dtype=torch.int64, device=keys.device)
     kk = key_kind(keys) if row_hash is None else K_ROWID
-    _check(lib().dpk_combine(_ptr(keys), kk, _ptr(row_hash), _ptr(vals), val_kind(vals), n, OPS[op], P,
+    src_k, src_v = keys, vals
+    if rows is not None:
+        if rows.dim() != 2 or rows.shape[1] != 2 or rows.shape[0] != n or keys.element_size() != vals.element_size():
+            raise ValueError("rows must be the packed [n, 2] buffer of the key and value columns")
+        kk |= K_PACKED
+        src_k, src_v = rows, None
+    _check(lib().dpk_combine(_ptr(src_k), kk, _ptr(row_hash), _ptr(src_v), val_kind(vals), n, OPS[op], P,
                              _ptr(thr), nthr, sub_bits, part_first, nparts, nsrc, _ptr(bucket_rows), _ptr(out_keys),
                              _ptr(out_vals), _ptr(out_offsets), _ptr(out_counts), _ptr(ws), ws_bytes,
                              _stream()))

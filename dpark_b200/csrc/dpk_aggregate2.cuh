@@ -225,7 +225,9 @@ __device__ __forceinline__ uint32_t ag2_slot(const uint32_t (&slots)[3], int j) 
 // order; the rows inside one still come in run-to-run varying order, as the unordered multisplits deliver them).
 // With hundreds of resident CTAs all finishing equal-sized buckets in lockstep, the look-back waits for the SLOWEST of its nearest predecessors every time, and a wider look-back window does not help; the atomic costs a fixed L2 round trip, no waiting on other CTAs, and lifts the
 // in-order requirement, so the next ticket and its row range are prefetched a bucket ahead.
-template <typename KeyT, typename ValT, typename AccT, int MINB, bool CURSOR, bool BATCHED, bool FAST_ONLY = false>
+// PACKED: the fine buckets are packed records (keys: PackedRow array, vals unused) -- one load per row
+template <typename KeyT, typename ValT, typename AccT, int MINB, bool CURSOR, bool BATCHED, bool FAST_ONLY = false,
+          bool PACKED = false>
 __global__ void __launch_bounds__(AG2_THREADS, MINB)
 k_smem_aggregate2(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, int op,
                   const int64_t *__restrict__ fine_off, int32_t nfine, int32_t fine_per_part,
@@ -275,7 +277,16 @@ k_smem_aggregate2(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, 
 #pragma unroll
         for (int j = 0; j < NI; j++) {
             const int i = j * AG2_THREADS + (int)threadIdx.x;
-            if (i < w) { kr[j] = keys[g0 + i]; vr[j] = vals[g0 + i]; }
+            if (i < w) {
+                if constexpr (PACKED) {
+                    const PackedRow<KeyT, ValT> r = reinterpret_cast<const PackedRow<KeyT, ValT> *>(keys)[g0 + i];
+                    kr[j] = r.k;
+                    vr[j] = r.v;
+                } else {
+                    kr[j] = keys[g0 + i];
+                    vr[j] = vals[g0 + i];
+                }
+            }
         }
         between();
 #pragma unroll

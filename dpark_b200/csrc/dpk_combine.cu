@@ -220,20 +220,20 @@ k_tbl_init(Slot *__restrict__ table, const int64_t *__restrict__ tbl_total, int6
 }
 
 // n is the length of the buffer; *rows_total (k_tbl_plan's part_off[nparts]) the rows seg_rows describes, the only
-// ones the table regions are sized for
+// ones the table regions are sized for.  row_stride: elements from one row to the next (2: packed rows, vals = keys + 1)
 template <typename KeyT, typename ValT, typename AccT>
 __global__ void __launch_bounds__(CB_THREADS)
 k_tbl_insert(const KeyT *__restrict__ keys, const int64_t *__restrict__ aux, const ValT *__restrict__ vals,
              int64_t n, const int64_t *__restrict__ rows_total, int op, PartFn f, int32_t bucket_first, int32_t F,
              const int64_t *__restrict__ tbl_off, Slot *__restrict__ table, Slot *__restrict__ side,
-             int32_t *__restrict__ side_used) {
+             int32_t *__restrict__ side_used, int64_t row_stride) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     const int64_t rows = min(n, *rows_total);
     for (; i < rows; i += stride) {
-        const KeyT key = keys[i];
+        const KeyT key = keys[i * row_stride];
         const int64_t kb = key_bits<KeyT>(key);
-        const AccT v = (AccT)vals[i];
+        const AccT v = (AccT)vals[i * row_stride];
         Slot *s;
         if (kb == kEmpty) {
             s = side;
@@ -322,7 +322,7 @@ k_bucket_reduce(const KeyT *__restrict__ keys, const int64_t *__restrict__ aux, 
                 const int64_t *__restrict__ tbl_off, Slot *__restrict__ table, Slot *__restrict__ side,
                 int32_t *__restrict__ side_used, const int64_t *__restrict__ part_offsets,
                 KeyT *__restrict__ out_keys, int64_t *__restrict__ out_vals,
-                unsigned long long *__restrict__ out_counts, int *__restrict__ bucket_counter) {
+                unsigned long long *__restrict__ out_counts, int *__restrict__ bucket_counter, int64_t row_stride) {
     cg::cluster_group cluster = cg::this_cluster();
     const unsigned crank = cluster.block_rank();
     __shared__ int s_bucket;
@@ -349,8 +349,8 @@ k_bucket_reduce(const KeyT *__restrict__ keys, const int64_t *__restrict__ aux, 
             const int64_t r0 = seg_start[(int64_t)s * F + b];
             const int64_t rn = seg_rows[(int64_t)s * F + b];
             for (int64_t i = tid_c; i < rn; i += nth_c) {
-                const int64_t kb = key_bits<KeyT>(keys[r0 + i]);
-                const AccT v = (AccT)vals[r0 + i];
+                const int64_t kb = key_bits<KeyT>(keys[(r0 + i) * row_stride]);
+                const AccT v = (AccT)vals[(r0 + i) * row_stride];
                 Slot *sl;
                 if (kb == kEmpty) {
                     sl = side;
@@ -463,6 +463,7 @@ int g_agg_target_rows = 2048;        // rows per fine bucket the split aims for 
 
 struct Ctx {
     int key_kind, val_bytes;
+    bool packed;        // the input rows are packed records (keys: the records, vals = keys + one key width)
     int64_t *fine_off;
     unsigned long long *fb_state;
     int *part_err;
@@ -497,8 +498,13 @@ static int dispatch_op(const Ctx &c) {
         fine.row_hash = c.aux;
         KeyT *rekeys = (KeyT *)c.table;
         ValT *revals = (ValT *)((char *)c.table + (size_t)c.n * 8);
+        // same-width rows leave the second-level split as packed records when the merge that follows reads them (the
+        // default launch pair below): one 16- or 8-byte load per row there, one bulk store per fine-bucket run here
+        constexpr bool same_width = sizeof(KeyT) == sizeof(ValT);
+        const bool pack_fine = same_width && g_agg_impl == 1 && !g_agg_pipe && g_agg_cursor && !g_agg_batched && g_agg_split;
+        const int pack = (c.packed ? PK_IN : 0) | (pack_fine ? PK_OUT : 0);
         int rc = seg_multisplit(c.keys, c.key_kind, c.vals, (int32_t)sizeof(ValT), c.n, fine, c.F, c.nsrc, c.seg_start,
-                                c.seg_rows, rekeys, revals, c.fine_off, c.seg_ws, c.seg_ws_bytes, c.st);
+                                c.seg_rows, rekeys, revals, c.fine_off, c.seg_ws, c.seg_ws_bytes, c.st, false, pack);
         if (rc) return rc;
         const int32_t nfine = c.F * S2;
         int grid = sm_count() * 8;
@@ -553,6 +559,14 @@ static int dispatch_op(const Ctx &c) {
                 // registers); oversized buckets are listed and merged by the full kernel in a second, usually empty launch
                 auto fast = g_agg_ctas == 4 ? k_smem_aggregate2<KeyT, ValT, AccT, 4, true, false, true>
                                             : k_smem_aggregate2<KeyT, ValT, AccT, 3, true, false, true>;
+                auto aggb = k_smem_aggregate2<KeyT, ValT, AccT, 3, true, false>;
+                if constexpr (same_width) {
+                    if (pack_fine) {   // the fine buckets are packed records
+                        fast = g_agg_ctas == 4 ? k_smem_aggregate2<KeyT, ValT, AccT, 4, true, false, true, true>
+                                               : k_smem_aggregate2<KeyT, ValT, AccT, 3, true, false, true, true>;
+                        aggb = k_smem_aggregate2<KeyT, ValT, AccT, 3, true, false, false, true>;
+                    }
+                }
                 DPK_CUDA_TRY(cudaFuncSetAttribute(fast, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
                 int *big_count = c.part_err + c.nparts, *list_counter = c.part_err + c.nparts + 1;
                 int *big_list = reinterpret_cast<int *>(c.fb_state);          // nfine * 8 bytes: idle in cursor mode
@@ -560,7 +574,6 @@ static int dispatch_op(const Ctx &c) {
                     rekeys, revals, c.op, c.fine_off, nfine, (1 << c.f.sub_bits) * S2, c.part_off,
                     (KeyT *)c.out_keys, c.out_vals, (long long *)c.out_counts, c.fb_state, c.bucket_counter, c.part_err,
                     nullptr, nullptr, timing, big_list, big_count));
-                auto aggb = k_smem_aggregate2<KeyT, ValT, AccT, 3, true, false>;
                 DPK_CUDA_TRY(cudaFuncSetAttribute(aggb, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
                 DPK_LAUNCH("smem_aggregate_big", c.st, aggb<<<sm_count() * 2, AG2_THREADS, smem2, c.st>>>(
                     rekeys, revals, c.op, c.fine_off, nfine, (1 << c.f.sub_bits) * S2, c.part_off,
@@ -598,7 +611,7 @@ static int dispatch_op(const Ctx &c) {
         DPK_LAUNCH("bucket_reduce", c.st, kern<<<nclusters * BR_CLUSTER, BR_THREADS, 0, c.st>>>(
             (const KeyT *)c.keys, c.aux, (const ValT *)c.vals, c.op, ident, c.f.sub_bits, c.F, c.nsrc,
             c.seg_start, c.seg_rows, c.tbl_off, c.table, c.side, c.side_used, c.part_off, (KeyT *)c.out_keys,
-            c.out_vals, c.out_counts, c.bucket_counter));
+            c.out_vals, c.out_counts, c.bucket_counter, c.packed ? 2 : 1));
     } else {
         DPK_LAUNCH("tbl_init", c.st, k_tbl_init<<<grid_cap(c.max_slots, CB_THREADS, 16), CB_THREADS, 0, c.st>>>(
             c.table, c.tbl_off + c.F, ident));
@@ -606,7 +619,7 @@ static int dispatch_op(const Ctx &c) {
             DPK_LAUNCH("tbl_insert", c.st, k_tbl_insert<KeyT, ValT, AccT><<<grid_cap(c.n, CB_THREADS, 16), CB_THREADS, 0, c.st>>>(
                 (const KeyT *)c.keys, c.aux, (const ValT *)c.vals, c.n, c.part_off + c.nparts, c.op, c.f,
                 c.part_first << c.f.sub_bits,
-                c.F, c.tbl_off, c.table, c.side, c.side_used));
+                c.F, c.tbl_off, c.table, c.side, c.side_used, c.packed ? 2 : 1));
         }
         size_t sh = (size_t)((c.nparts + 1) & ~1) * 4 + (size_t)c.nparts * 8;
         DPK_LAUNCH("tbl_compact", c.st, k_tbl_compact<KeyT><<<grid_cap(c.max_slots, CB_THREADS * 4, 8), CB_THREADS, sh, c.st>>>(
@@ -788,6 +801,16 @@ int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const vo
         return fail(DPK_ERR_INVALID, "bad partition range first=%d n=%d P=%d", part_first, nparts, P);
     if (nsrc < 1) return fail(DPK_ERR_INVALID, "nsrc must be >= 1");
     if (!seg_rows || !out_counts || !out_offsets || !ws) return fail(DPK_ERR_INVALID, "NULL pointer");
+    const bool packed = key_kind >= 0 && (key_kind & DPK_K_PACKED);
+    if (packed) {   // keys points at packed records: the value of row i follows its key
+        key_kind &= ~DPK_K_PACKED;
+        const int kw = (key_kind == DPK_K_I32 || key_kind == DPK_K_F32) ? 4 : 8;
+        const int vw = (val_kind == DPK_V_I32 || val_kind == DPK_V_F32) ? 4 : 8;
+        if (vals) return fail(DPK_ERR_INVALID, "packed rows: vals must be NULL");
+        if (kw != vw) return fail(DPK_ERR_UNSUPPORTED, "packed rows need values as wide as the keys");
+        if ((uintptr_t)keys % (2 * kw)) return fail(DPK_ERR_INVALID, "packed rows must be aligned to their %d-byte size", 2 * kw);
+        vals = keys ? (const char *)keys + kw : nullptr;
+    }
     if (n > 0 && (!keys || !vals || !out_keys || !out_vals)) return fail(DPK_ERR_INVALID, "NULL pointer");
     Ctx c;
     int rc = make_partfn(P, thresholds, nthr, sub_bits, &c.f);
@@ -798,6 +821,7 @@ int dpk_combine(const void *keys, int key_kind, const int64_t *key_aux, const vo
     if (ws_bytes < dpk_combine_workspace_bytes(n, c.F, nsrc))
         return fail(DPK_ERR_WORKSPACE, "workspace needs %lld B, got %lld", (long long)dpk_combine_workspace_bytes(n, c.F, nsrc), (long long)ws_bytes);
     c.keys = keys; c.vals = vals; c.n = n; c.op = op; c.aux = key_aux; c.key_kind = key_kind; c.val_bytes = 0;
+    c.packed = packed;
     if (key_kind == DPK_K_ROWID && n > 0 && !key_aux) return fail(DPK_ERR_INVALID, "DPK_K_ROWID needs key_aux (the per-row hash column)");
     c.part_first = part_first; c.nparts = nparts; c.nsrc = nsrc; c.seg_rows = seg_rows;
     c.max_slots = max_slots_for(n, c.F);

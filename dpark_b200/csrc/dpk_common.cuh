@@ -226,11 +226,23 @@ int make_partfn(int32_t P, const int64_t *thresholds, int32_t nthr, int32_t sub_
 // bucket b (rows in nsrc segments seg_start/seg_rows[s][b] of the input) is split into
 // fine.nbuckets() fine buckets; output rows are bucket-major then fine-bucket-major and
 // fine_off[F1 * S2 + 1] delimits the fine buckets.  keys/vals: device; st-ordered.
+// pack: PK_OUT = write packed rows (out_keys: PackedRow array, out_vals unused), PK_IN = read packed rows (keys:
+// PackedRow array, vals unused); both need key and value columns of the same width.
 int64_t seg_multisplit_ws_bytes(int64_t n, int32_t F1, int32_t S2, int32_t nsrc);
 int seg_multisplit(const void *keys, int key_kind, const void *vals, int32_t val_bytes, int64_t n,
                    const PartFn &fine, int32_t F1, int32_t nsrc, const int64_t *seg_start,
                    const int64_t *seg_rows, void *out_keys, void *out_vals, int64_t *fine_off, void *ws,
-                   int64_t ws_bytes, cudaStream_t st, bool stable = false);
+                   int64_t ws_bytes, cudaStream_t st, bool stable = false, int pack = 0);
+
+// Packed shuffle rows (DPK_K_PACKED): one record per row, key then value, for key and value columns of the same
+// width -- 16-byte records for 8-byte columns, 8-byte records for 4-byte ones.  A multisplit that writes records stores
+// one bucket run per bucket instead of one per column, and a reader fetches a row with one load.
+constexpr int PK_OUT = 1, PK_IN = 2;
+template <typename KeyT, typename ValT>
+struct __align__(2 * sizeof(KeyT)) PackedRow {
+    KeyT k;
+    ValT v;
+};
 
 // murmur3 fmix64 -- slot hash for the reduce-side tables in HBM (implementations 0/1; not part of the
 // reference semantics; only spreads keys over table slots)

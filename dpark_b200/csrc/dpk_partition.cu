@@ -74,6 +74,7 @@ struct Plan {
     int64_t L;  // rows per CTA, multiple of PT_TILE
     SegTab seg;
     const char *label_count = nullptr, *label_scatter = nullptr;  // profiling labels (default: part_* / seg_*)
+    int pack = 0;   // PK_IN | PK_OUT: packed rows in / out (same-width key and value columns)
 };
 
 static Plan make_plan(int64_t n) {
@@ -149,7 +150,8 @@ __device__ __forceinline__ int block_excl_scan(int v, int *s_warp, int *total) {
 }
 
 // ------------------------------------------------------------------ count
-template <typename KeyT, int PRE>
+// PIN: the rows are packed records (key then a value of the key's width): the key of row i is element 2 * i
+template <typename KeyT, int PRE, bool PIN = false>
 __global__ void __launch_bounds__(PT_THREADS)
 k_part_count(const KeyT *__restrict__ keys, int64_t n, int64_t L, PartFn f,
              int32_t *__restrict__ tile_counts, int32_t T, SegTab seg, int count_mode) {
@@ -175,7 +177,7 @@ k_part_count(const KeyT *__restrict__ keys, int64_t n, int64_t L, PartFn f,
         for (; i0 + (int64_t)PT_THREADS * U <= end; i0 += (int64_t)PT_THREADS * U) {
             KeyT k[U];
 #pragma unroll
-            for (int u = 0; u < U; u++) k[u] = keys[i0 + (int64_t)u * PT_THREADS + threadIdx.x];
+            for (int u = 0; u < U; u++) k[u] = keys[(i0 + (int64_t)u * PT_THREADS + threadIdx.x) * (PIN ? 2 : 1)];
 #pragma unroll
             for (int u = 0; u < U; u++) atomicAdd(&wh[f.bucket(key_hash<KeyT, PRE>(k[u], f))], 1);
         }
@@ -187,7 +189,7 @@ k_part_count(const KeyT *__restrict__ keys, int64_t n, int64_t L, PartFn f,
         for (int u = 0; u < U; u++) {
             int64_t i = i0 + (int64_t)u * PT_THREADS + threadIdx.x;
             ok[u] = i < end;
-            k[u] = ok[u] ? keys[i] : KeyT(0);
+            k[u] = ok[u] ? keys[i * (PIN ? 2 : 1)] : KeyT(0);
         }
 #pragma unroll
         for (int u = 0; u < U; u++) {
@@ -284,13 +286,15 @@ static ScatterSmem scatter_smem(int kb, int vb, int32_t P, bool ptr_mode, int ti
 // ITEMS rows per thread and tile: 16 (4096-row tiles, 2 CTAs per SM) or 8 (2048-row tiles, half the
 // registers and shared memory, 4 CTAs per SM -- more warps to hide the phase barriers; bucket runs
 // inside a tile are half as long).  The CTA's row range comes from the plan in PT_TILE units either way.
-template <typename KeyT, typename ValT, int PRE, int ITEMS>
+// PK (PK_IN | PK_OUT bits, plain and segmented destinations only): rows are read from / written as packed records.
+template <typename KeyT, typename ValT, int PRE, int ITEMS, int PK = 0>
 __global__ void __launch_bounds__(PT_THREADS, ITEMS == 16 ? 2 : 4)
 k_part_scatter(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, int64_t n, int64_t L,
                PartFn f, const int32_t *__restrict__ tile_off, int32_t T,
                const int64_t *__restrict__ bucket_base, KeyT *__restrict__ out_keys,
                ValT *__restrict__ out_vals, ScatterSmem lay, SegTab seg) {
     constexpr bool HAS_VAL = !std::is_same<ValT, NoVal>::value;
+    using Rec = PackedRow<KeyT, ValT>;
     constexpr int TILE = PT_THREADS * ITEMS;
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_warp[PT_WARPS];
@@ -334,12 +338,25 @@ k_part_scatter(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, int
         KeyT k[ITEMS];
         ValT v[ITEMS];
         const int64_t wbase = tile + (int64_t)warp * (32 * ITEMS) + lane;
+        if constexpr ((PK & PK_IN) != 0) {
 #pragma unroll
-        for (int j = 0; j < ITEMS; j++) {
-            int64_t idx = wbase + j * 32;
-            k[j] = idx < end ? keys[idx] : KeyT(0);
+            for (int j = 0; j < ITEMS; j++) {
+                int64_t idx = wbase + j * 32;
+                k[j] = KeyT(0);
+                if (idx < end) {
+                    const Rec r = reinterpret_cast<const Rec *>(keys)[idx];
+                    k[j] = r.k;
+                    v[j] = r.v;
+                }
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < ITEMS; j++) {
+                int64_t idx = wbase + j * 32;
+                k[j] = idx < end ? keys[idx] : KeyT(0);
+            }
         }
-        if constexpr (HAS_VAL) {
+        if constexpr (HAS_VAL && (PK & PK_IN) == 0) {
 #pragma unroll
             for (int j = 0; j < ITEMS; j++) {
                 int64_t idx = wbase + j * 32;
@@ -421,7 +438,9 @@ k_part_scatter(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, int
         for (int i = threadIdx.x; i < rows; i += PT_THREADS) {
             const int p = s_pid[i];
             const int64_t dst = s_gpos[p] + (int64_t)(i - s_tstart[p]);
-            if (seg.key_ptrs) {  // pointer mode: the bucket's destination may be a peer GPU
+            if constexpr ((PK & PK_OUT) != 0) {
+                reinterpret_cast<Rec *>(out_keys)[dst] = Rec{s_key[i], s_val[i]};
+            } else if (seg.key_ptrs) {  // pointer mode: the bucket's destination may be a peer GPU
                 reinterpret_cast<KeyT *>(s_kptr[p])[dst] = s_key[i];
                 if constexpr (HAS_VAL) reinterpret_cast<ValT *>(s_vptr[p])[dst] = s_val[i];
             } else {
@@ -508,7 +527,10 @@ __device__ __forceinline__ int bucket_of(const PartFn &f, int64_t h) {
     }
 }
 
-template <typename KeyT, typename ValT, int PRE, int NT, int FMODE, bool PTRS = false>
+// PK (PK_IN | PK_OUT bits, not with PTRS): rows are read from / staged and written as packed records.  A packed tile is
+// one array of records: every bucket run leaves with ONE bulk store, issued by one thread per bucket, and with 16-byte
+// records every run starts and ends on a 16-byte boundary (no head or tail stores).
+template <typename KeyT, typename ValT, int PRE, int NT, int FMODE, bool PTRS = false, int PK = 0>
 __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2)
 k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals, int64_t n, int64_t L,
                     PartFn f, const int32_t *__restrict__ tile_off, int32_t T,
@@ -522,11 +544,17 @@ k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals
     constexpr int NW = NT / 32;
     constexpr int AK = 16 / (int)sizeof(KeyT);
     constexpr int AV = HAS_VAL ? 16 / (int)sizeof(typename std::conditional<HAS_VAL, ValT, int64_t>::type) : 1;
+    constexpr bool PIN = (PK & PK_IN) != 0, POUT = (PK & PK_OUT) != 0;
+    using Rec = PackedRow<KeyT, ValT>;
+    constexpr int AR = 16 / (int)sizeof(Rec);
+    static_assert(PK == 0 || (HAS_VAL && !PTRS && sizeof(KeyT) == sizeof(ValT)), "packed rows: same-width key and value, plain or segmented mode");
     extern __shared__ __align__(128) unsigned char smem_bulk[];
     unsigned char *smem = smem_bulk;
     __shared__ int s_warp[NW];
     KeyT *s_key = reinterpret_cast<KeyT *>(smem + lay.key_off);
     ValT *s_val = reinterpret_cast<ValT *>(smem + lay.val_off);
+    Rec *s_rec = reinterpret_cast<Rec *>(smem + lay.key_off);                 // POUT: the staging tile holds records
+    Rec *out_rec = reinterpret_cast<Rec *>(out_keys);
     int64_t *s_gpos = reinterpret_cast<int64_t *>(smem + lay.gpos_off);
     uint32_t *s_cnt = reinterpret_cast<uint32_t *>(smem + lay.cnt_off);      // [2][P]
     int32_t *s_sk = reinterpret_cast<int32_t *>(smem + lay.sk_off);          // start of bucket p's key run in the staging tile
@@ -565,6 +593,20 @@ k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals
     ValT v[ITEMS];
     // rows of the tile this thread holds: row j of warp w's lane l = tile + w * 32 * ITEMS + j * 32 + l
     auto load_tile = [&](int64_t tile) {
+        if constexpr (PIN) {   // one 8- or 16-byte load per row
+            const Rec *rp = reinterpret_cast<const Rec *>(keys) + tile + warp * (32 * ITEMS) + lane;
+            const int left = (int)min((int64_t)TILE, end - tile) - warp * (32 * ITEMS) - lane;
+#pragma unroll
+            for (int j = 0; j < ITEMS; j++) {
+                k[j] = KeyT(0);
+                if (j * 32 < left) {
+                    const Rec r = rp[j * 32];
+                    k[j] = r.k;
+                    v[j] = r.v;
+                }
+            }
+            return;
+        }
         const KeyT *kp = keys + tile + warp * (32 * ITEMS) + lane;
         if (tile + TILE <= end) {
 #pragma unroll
@@ -625,6 +667,13 @@ k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals
             int run = block_excl_scan<NW>(sum, s_warp, &tot);
             for (int i = b; i < min(b + E, P); i++) {
                 const int64_t g = s_gpos[i];
+                if constexpr (POUT) {
+                    const uint32_t gr = (uint32_t)(((uintptr_t)(out_rec + g)) / sizeof(Rec));
+                    const int baser = run + i * (AR - 1);
+                    s_sk[i] = baser + (int)((gr - (uint32_t)baser) & (uint32_t)(AR - 1));
+                    run += (int)cnt[i];
+                    continue;
+                }
                 const uint32_t gk = (uint32_t)(((uintptr_t)(out_keys + g)) / sizeof(KeyT));
                 const int basek = run + i * (AK - 1);
                 s_sk[i] = basek + (int)((gk - (uint32_t)basek) & (uint32_t)(AK - 1));
@@ -643,8 +692,12 @@ k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals
         for (int j = 0; j < ITEMS; j++) {
             const int p = (int)(pr[j] >> 16), r = (int)(pr[j] & 0xffffu);
             if (p != 0xffff) {
-                s_key[s_sk[p] + r] = k[j];
-                if constexpr (HAS_VAL) s_val[s_sv[p] + r] = v[j];
+                if constexpr (POUT) {
+                    s_rec[s_sk[p] + r] = Rec{k[j], v[j]};
+                } else {
+                    s_key[s_sk[p] + r] = k[j];
+                    if constexpr (HAS_VAL) s_val[s_sv[p] + r] = v[j];
+                }
             }
         }
         // registers are free: fetch the next tile now, its latency hides behind the barrier and the copy-out
@@ -654,8 +707,20 @@ k_part_scatter_bulk(const KeyT *__restrict__ keys, const ValT *__restrict__ vals
 
         // ---- copy-out: bucket runs leave through the TMA.  With values, lane pairs share a bucket (even lane: key
         //      run, odd lane: value run) so that every thread issues at most one bulk store per round: the issue
-        //      rate of one thread bounds the bulk-store rate below 512-byte runs (scripts/microbench/smem_ops.cu)
-        if constexpr (HAS_VAL) {
+        //      rate of one thread bounds the bulk-store rate below 512-byte runs (scripts/microbench/smem_ops.cu).
+        //      Packed records: one run per bucket, one thread per bucket.
+        if constexpr (POUT) {
+            const uint32_t rec_addr = key_addr;
+            for (int p = threadIdx.x; p < P; p += NT) {
+                const int c = (int)cnt[p];
+                if (c) {
+                    const int64_t g = s_gpos[p];
+                    flush_run<Rec>(out_rec, g, s_rec, rec_addr, s_sk[p], c);
+                    s_gpos[p] = g + c;
+                    cnt[p] = 0;
+                }
+            }
+        } else if constexpr (HAS_VAL) {
             for (int q0 = 0; q0 < 2 * P; q0 += NT) {
                 const int q = q0 + (int)threadIdx.x;
                 const int p = q >> 1;
@@ -693,12 +758,14 @@ template <typename KeyT, int PRE>
 static int launch_count(const void *keys, int64_t n, const Plan &pl, const PartFn &f,
                         int32_t *tile_counts, cudaStream_t st) {
     size_t sh = (size_t)f.nbuckets() * sizeof(int32_t) * (f.nbuckets() <= PT_COUNT_PRIV ? PT_WARPS : 1);
-    DPK_LAUNCH(pl.label_count ? pl.label_count : (pl.seg.cbeg ? "seg_count" : "part_count"), st, k_part_count<KeyT, PRE><<<pl.T, PT_THREADS, sh, st>>>((const KeyT *)keys, n, pl.L, f, tile_counts, pl.T, pl.seg, g_count_mode));
+    auto kern = (pl.pack & PK_IN) ? k_part_count<KeyT, PRE, true> : k_part_count<KeyT, PRE, false>;
+    DPK_LAUNCH(pl.label_count ? pl.label_count : (pl.seg.cbeg ? "seg_count" : "part_count"), st, kern<<<pl.T, PT_THREADS, sh, st>>>((const KeyT *)keys, n, pl.L, f, tile_counts, pl.T, pl.seg, g_count_mode));
     return DPK_OK;
 }
 
 static int dispatch_count(const void *keys, int key_kind, int64_t n, const Plan &pl, const PartFn &f,
                           int32_t *tile_counts, cudaStream_t st) {
+    if (key_kind >= 0) key_kind &= ~DPK_K_PACKED;                   // nor about the layout the scatter writes
     if (key_kind >= DPK_K_UNORDERED) key_kind -= DPK_K_UNORDERED;  // the histogram does not care about order
     switch (key_kind) {
     case -1: return launch_count<int64_t, true>(keys, n, pl, f, tile_counts, st);
@@ -721,6 +788,11 @@ static int launch_scatter_items(const void *keys, const void *vals, int64_t n, c
     constexpr int vb = std::is_same<ValT, NoVal>::value ? 0 : (int)sizeof(ValT);
     ScatterSmem lay = scatter_smem((int)sizeof(KeyT), vb, f.nbuckets(), pl.seg.key_ptrs != nullptr, PT_THREADS * ITEMS);
     auto kern = k_part_scatter<KeyT, ValT, PRE, ITEMS>;
+    if constexpr (vb == (int)sizeof(KeyT) && ITEMS == 16) {
+        if (pl.pack == PK_OUT) kern = k_part_scatter<KeyT, ValT, PRE, ITEMS, PK_OUT>;
+        else if (pl.pack == PK_IN) kern = k_part_scatter<KeyT, ValT, PRE, ITEMS, PK_IN>;
+        else if (pl.pack == (PK_IN | PK_OUT)) kern = k_part_scatter<KeyT, ValT, PRE, ITEMS, PK_IN | PK_OUT>;
+    }
     if (lay.total > 227 * 1024)
         return fail(DPK_ERR_UNSUPPORTED, "%d buckets need %lld B of shared memory", f.nbuckets(), (long long)lay.total);
     DPK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
@@ -736,6 +808,30 @@ static int launch_scatter_bulk(const void *keys, const void *vals, int64_t n, co
                                const int32_t *tile_off, const int64_t *bucket_base, void *out_keys,
                                void *out_vals, cudaStream_t st) {
     constexpr int vb = std::is_same<ValT, NoVal>::value ? 0 : (int)sizeof(ValT);
+    if constexpr (vb == (int)sizeof(KeyT)) {
+        if (pl.pack) {
+            // packed rows: 8192-row tiles (1024 threads) always -- a tile of records takes the shared memory of a tile of
+            // two columns and its runs are one bulk store each.  Packed input only comes from the reduce side, whose
+            // fine bucket function is the second-level split (FMODE 2).
+            const int fmode = f.mode == 5 ? 2 : ((f.mode == 0 || f.mode == 1) ? 1 : 0);
+            BulkSmem lay = bulk_smem(2 * (int)sizeof(KeyT), 0, f.nbuckets(), 8192);
+            auto kern = fmode == 2 ? k_part_scatter_bulk<KeyT, ValT, PRE, 1024, 2, false, PK_OUT>
+                      : fmode == 1 ? k_part_scatter_bulk<KeyT, ValT, PRE, 1024, 1, false, PK_OUT>
+                                   : k_part_scatter_bulk<KeyT, ValT, PRE, 1024, 0, false, PK_OUT>;
+            if (pl.pack & PK_IN) {
+                if (fmode != 2) return fail(DPK_ERR_UNSUPPORTED, "packed input needs the second-level split");
+                kern = (pl.pack & PK_OUT) ? k_part_scatter_bulk<KeyT, ValT, PRE, 1024, 2, false, PK_IN | PK_OUT>
+                                          : k_part_scatter_bulk<KeyT, ValT, PRE, 1024, 2, false, PK_IN>;
+                if (!(pl.pack & PK_OUT)) lay = bulk_smem((int)sizeof(KeyT), vb, f.nbuckets(), 8192);
+            }
+            DPK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+            DPK_LAUNCH(pl.label_scatter ? pl.label_scatter : (pl.seg.cbeg ? "seg_scatter" : "part_scatter"), st,
+                       kern<<<pl.T, 1024, (size_t)lay.total, st>>>((const KeyT *)keys, (const ValT *)vals, n, pl.L, f,
+                                                                  tile_off, pl.T, bucket_base, (KeyT *)out_keys,
+                                                                  (ValT *)out_vals, lay, pl.seg));
+            return DPK_OK;
+        }
+    }
     // dpk_set_option("scatter_threads"): 512 (default; 8 rows per thread, 4096-row tiles, 2 CTAs per SM), 256 (16 rows
     // per thread) or 1024 (8192-row tiles, 1 CTA per SM)
     int nt = g_scatter_threads;
@@ -781,12 +877,15 @@ static int launch_scatter(const void *keys, const void *vals, int64_t n, const P
     Plan pl = pl_in;
     if (pl.seg.unordered == 2) {  // unordered + plain/segmented destination: the TMA bulk-store kernel
         constexpr int vb = std::is_same<ValT, NoVal>::value ? 0 : (int)sizeof(ValT);
-        if (bulk_smem((int)sizeof(KeyT), vb, f.nbuckets(), PT_TILE, pl.seg.key_ptrs != nullptr).total <= 110 * 1024)
+        const bool fits = (pl.pack & PK_OUT) ? bulk_smem(2 * (int)sizeof(KeyT), 0, f.nbuckets(), 8192).total <= 220 * 1024
+                        : pl.pack ? bulk_smem((int)sizeof(KeyT), vb, f.nbuckets(), 8192).total <= 220 * 1024
+                                  : bulk_smem((int)sizeof(KeyT), vb, f.nbuckets(), PT_TILE, pl.seg.key_ptrs != nullptr).total <= 110 * 1024;
+        if (fits)
             return launch_scatter_bulk<KeyT, ValT, PRE>(keys, vals, n, pl, f, tile_off, bucket_base, out_keys, out_vals, st);
         pl.seg.unordered = (f.nbuckets() % 2 == 0) ? 1 : 0;  // too many buckets for two resident CTAs: the round-1 kernel
     }
-    // dpk_set_option("scatter_items"): 16 or 8 rows per thread and tile (A/B switch)
-    if (g_scatter_items == 8)
+    // dpk_set_option("scatter_items"): 16 or 8 rows per thread and tile (A/B switch; packed rows: 16)
+    if (g_scatter_items == 8 && !pl.pack)
         return launch_scatter_items<KeyT, ValT, PRE, 8>(keys, vals, n, pl, f, tile_off, bucket_base, out_keys, out_vals, st);
     return launch_scatter_items<KeyT, ValT, PRE, 16>(keys, vals, n, pl, f, tile_off, bucket_base, out_keys, out_vals, st);
 }
@@ -795,7 +894,14 @@ template <typename KeyT, int PRE>
 static int dispatch_val(const void *keys, const void *vals, int32_t val_bytes, int64_t n, const Plan &pl,
                         const PartFn &f, const int32_t *tile_off, const int64_t *bucket_base,
                         void *out_keys, void *out_vals, cudaStream_t st) {
-    if (vals == nullptr || val_bytes == 0)
+    if (pl.pack) {
+        if (vals == nullptr && !(pl.pack & PK_IN)) return fail(DPK_ERR_INVALID, "packed rows need a value column");
+        if (val_bytes != (int)sizeof(KeyT)) return fail(DPK_ERR_UNSUPPORTED, "packed rows need values as wide as the keys (%d B), got %d B", (int)sizeof(KeyT), val_bytes);
+        if (pl.seg.key_ptrs) return fail(DPK_ERR_UNSUPPORTED, "packed rows are not written through pointer tables");
+        if (((pl.pack & PK_OUT) && ((uintptr_t)out_keys % (2 * sizeof(KeyT)))) || ((pl.pack & PK_IN) && ((uintptr_t)keys % (2 * sizeof(KeyT)))))
+            return fail(DPK_ERR_INVALID, "packed rows must be aligned to their %d-byte size", 2 * (int)sizeof(KeyT));
+    }
+    if ((vals == nullptr && !(pl.pack & PK_IN)) || val_bytes == 0)
         return launch_scatter<KeyT, NoVal, PRE>(keys, nullptr, n, pl, f, tile_off, bucket_base, out_keys, nullptr, st);
     if (val_bytes == 8)
         return launch_scatter<KeyT, int64_t, PRE>(keys, vals, n, pl, f, tile_off, bucket_base, out_keys, out_vals, st);
@@ -808,6 +914,10 @@ static int dispatch_scatter(const void *keys, int key_kind, const void *vals, in
                             const Plan &pl_in, const PartFn &f, const int32_t *tile_off,
                             const int64_t *bucket_base, void *out_keys, void *out_vals, cudaStream_t st) {
     Plan pl = pl_in;
+    if (key_kind >= 0 && (key_kind & DPK_K_PACKED)) {  // packed output
+        key_kind &= ~DPK_K_PACKED;
+        pl.pack |= PK_OUT;
+    }
     if (key_kind >= DPK_K_UNORDERED) {  // caller does not need input order inside a bucket
         key_kind -= DPK_K_UNORDERED;
         if (f.nbuckets() % 2 == 0) pl.seg.unordered = 1;  // packed 16-bit counter pairs need an even bucket count
@@ -934,7 +1044,7 @@ int64_t seg_multisplit_ws_bytes(int64_t n, int32_t F1, int32_t S2, int32_t nsrc)
 int seg_multisplit(const void *keys, int key_kind, const void *vals, int32_t val_bytes, int64_t n,
                    const PartFn &fine, int32_t F1, int32_t nsrc, const int64_t *seg_start,
                    const int64_t *seg_rows, void *out_keys, void *out_vals, int64_t *fine_off, void *ws,
-                   int64_t ws_bytes, cudaStream_t st, bool stable) {
+                   int64_t ws_bytes, cudaStream_t st, bool stable, int pack) {
     const int32_t S2 = fine.nbuckets();
     if (ws_bytes < seg_multisplit_ws_bytes(n, F1, S2, nsrc)) return fail(DPK_ERR_WORKSPACE, "segmented multisplit workspace too small");
     const int64_t maxc = seg_max_chunks(n, F1, nsrc);
@@ -952,6 +1062,7 @@ int seg_multisplit(const void *keys, int key_kind, const void *vals, int32_t val
     pl.L = 0;
     // the reduce side never needs the order of rows inside a fine bucket
     pl.seg = SegTab{cbeg, cend, ctotal, chunk_counts, chunk_off, nullptr, nullptr, (S2 % 2 == 0) ? 1 : (g_scatter_bulk ? 2 : 0)};
+    pl.pack = pack;
     if (stable) {   // radix passes of the group-by: rows of a fine bucket keep their order (warp-match ranking)
         pl.seg.unordered = 0;
         pl.label_count = "radix_count";

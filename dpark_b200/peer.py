@@ -170,6 +170,7 @@ def exchange_push(px, mo, need_host_count=False):
     sort buffers on the host).  The returned Received views the WHOLE receive buffer (`bound` rows);
     the rows actually received are what its segment matrix says."""
     G, rank, dev = px.world, px.rank, px.device
+    mo = mo.unpacked()     # the pushes move whole column blocks
     P, sb = mo.P, mo.sub_bits
     F = P << sb
     if mo.keys.dtype != px.keys.dtype or (mo.vals is not None and mo.vals.dtype != px.vals.dtype):

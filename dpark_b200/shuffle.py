@@ -93,11 +93,19 @@ def bind_to_gpu_numa_node(local_rank):
 
 
 class MapOutput(object):
-    """Bucket-major output of the map side on one rank: the alltoallv send buffer."""
-    __slots__ = ("keys", "vals", "offsets", "P", "sub_bits")
+    """Bucket-major output of the map side on one rank: the alltoallv send buffer.  rows: None, or the packed [n, 2]
+    buffer of (key, value) records that keys and vals are strided column views of (see map_side)."""
+    __slots__ = ("keys", "vals", "offsets", "P", "sub_bits", "rows")
 
-    def __init__(self, keys, vals, offsets, P, sub_bits):
+    def __init__(self, keys, vals, offsets, P, sub_bits, rows=None):
         self.keys, self.vals, self.offsets, self.P, self.sub_bits = keys, vals, offsets, P, sub_bits
+        self.rows = rows
+
+    def unpacked(self):
+        """This map output with contiguous key and value columns (an exchange between ranks moves columns)."""
+        if self.rows is None:
+            return self
+        return MapOutput(self.keys.contiguous(), self.vals.contiguous(), self.offsets, self.P, self.sub_bits)
 
 
 def _as_one(chunks):
@@ -124,8 +132,15 @@ def map_side(key_chunks, val_chunks, P, thresholds=None, prehashed=False, sub_bi
 
     key_chunks/val_chunks: lists of CUDA tensors (the rank's map splits in map_id
     order).  Rows of a bucket are ordered by (map split, position) -- the order
-    OrderedGroupByDiskHashMerger produces (dpark/shuffle.py:626-646)."""
+    OrderedGroupByDiskHashMerger produces (dpark/shuffle.py:626-646).
+
+    Packed rows: an unordered (reduceByKey) split of hashed keys with values of the key's width, whose exchange is the
+    identity (one rank, or inside local_only), writes one [n, 2] buffer of (key, value) records instead of two columns
+    -- the multisplit stores half as many, twice as long bucket runs and the reduce side reads one record per row.  The
+    MapOutput then carries that buffer as `rows`, and keys / vals are strided views of it."""
     F = P << sub_bits
+    packed = (unordered and val_chunks[0] is not None and _world() == 1
+              and nv.packable(key_chunks[0], val_chunks[0], prehashed))
     if len(key_chunks) > 1:
         # map splits that are consecutive slices of one buffer (the usual case: a batch copied to the device and
         # cut into map tasks) are partitioned in ONE launch pair: rows of a bucket stay in (split, position) order
@@ -134,7 +149,10 @@ def map_side(key_chunks, val_chunks, P, thresholds=None, prehashed=False, sub_bi
         if whole_k is not None and (val_chunks[0] is None or whole_v is not None) and whole_k.numel() < (1 << 31):
             key_chunks, val_chunks = [whole_k], [whole_v]
     if len(key_chunks) == 1:
-        k, v, off = nv.partition(key_chunks[0], val_chunks[0], P, thresholds, prehashed, sub_bits, row_hash, unordered)
+        k, v, off = nv.partition(key_chunks[0], val_chunks[0], P, thresholds, prehashed, sub_bits, row_hash, unordered,
+                                 packed)
+        if packed:
+            return MapOutput(*nv.packed_views(k, key_chunks[0].dtype, val_chunks[0].dtype), off, P, sub_bits, rows=k)
         return MapOutput(k, v, off, P, sub_bits)
     dev = key_chunks[0].device
     counts, wss = [], []
@@ -149,23 +167,31 @@ def map_side(key_chunks, val_chunks, P, thresholds=None, prehashed=False, sub_bi
     # base[m][b] = offsets[b] + rows of bucket b in earlier splits
     base = offsets[:-1].unsqueeze(0) + (torch.cumsum(cm, 0) - cm)
     n = sum(int(k.numel()) for k in key_chunks)
-    out_k = torch.empty(n, dtype=key_chunks[0].dtype, device=dev)
     has_v = val_chunks[0] is not None
-    out_v = torch.empty(n, dtype=val_chunks[0].dtype, device=dev) if has_v else None
+    if packed:
+        rows = nv.packed_rows(n, key_chunks[0].dtype, dev)
+        out_k, out_v = rows, None
+    else:
+        out_k = torch.empty(n, dtype=key_chunks[0].dtype, device=dev)
+        out_v = torch.empty(n, dtype=val_chunks[0].dtype, device=dev) if has_v else None
     for m, (k, v) in enumerate(zip(key_chunks, val_chunks)):
         nv.partition_scatter(k, v, P, base[m].contiguous(), out_k, out_v, wss[m], thresholds, prehashed, sub_bits,
                              row_hash, unordered)
+    if packed:
+        return MapOutput(*nv.packed_views(rows, key_chunks[0].dtype, val_chunks[0].dtype), offsets, P, sub_bits,
+                         rows=rows)
     return MapOutput(out_k, out_v, offsets, P, sub_bits)
 
 
 class Received(object):
     """Rows fetched for the partitions this rank owns.  keys/vals are laid out
     source-rank-major, then bucket-major; seg[s][b] = rows from source s for
-    local fine bucket b."""
-    __slots__ = ("keys", "vals", "seg", "part_first", "nparts", "sub_bits", "bound")
+    local fine bucket b.  rows: the packed buffer keys / vals view, when the rows arrived packed (MapOutput.rows)."""
+    __slots__ = ("keys", "vals", "seg", "part_first", "nparts", "sub_bits", "bound", "rows")
 
-    def __init__(self, keys, vals, seg, part_first, nparts, sub_bits, bound=False):
+    def __init__(self, keys, vals, seg, part_first, nparts, sub_bits, bound=False, rows=None):
         self.keys, self.vals, self.seg = keys, vals, seg
+        self.rows = rows
         self.part_first, self.nparts, self.sub_bits = part_first, nparts, sub_bits
         # bound: keys/vals are a whole receive buffer (an upper bound of the rows); the rows actually received are
         # seg.sum() and stay on the device (no host sync on the reduceByKey path)
@@ -195,7 +221,8 @@ def exchange(mo, group=None):
     P, sb = mo.P, mo.sub_bits
     if G == 1:
         seg = (mo.offsets[1:] - mo.offsets[:-1]).unsqueeze(0)
-        return Received(mo.keys, mo.vals, seg, 0, P, sb)
+        return Received(mo.keys, mo.vals, seg, 0, P, sb, rows=mo.rows)
+    mo = mo.unpacked()
     rank = dist.get_rank(group)
     F = P << sb
     blocks = [b << sb for b in owner_blocks(P, G)]                  # in fine buckets
@@ -227,7 +254,7 @@ def reduce_side(rx, op, P, thresholds=None):
         z = torch.zeros(1, dtype=torch.int64, device=dev)
         return rx.keys[:0], (rx.vals[:0] if rx.vals is not None else None), z, z[:0]
     return nv.combine(rx.keys, rx.vals, op, P, rx.seg.contiguous(), rx.part_first, rx.nparts, thresholds,
-                      rx.sub_bits)
+                      rx.sub_bits, rows=rx.rows)
 
 
 RADIX_BITS = 8
@@ -530,7 +557,7 @@ def combine_map_output(mo, op, thresholds=None):
     commutative; float sums are order-free up to the tolerance stated in DESIGN.md §7)."""
     P, sb = mo.P, mo.sub_bits
     seg = (mo.offsets[1:] - mo.offsets[:-1]).unsqueeze(0)
-    ok, ov, po, cnt = reduce_side(Received(mo.keys, mo.vals, seg, 0, P, sb), op, P, thresholds)
+    ok, ov, po, cnt = reduce_side(Received(mo.keys, mo.vals, seg, 0, P, sb, rows=mo.rows), op, P, thresholds)
     po_h, cnt_h = po.cpu().tolist(), cnt.cpu().tolist()           # host read: sizes of the compacted columns
     check_counts(cnt_h)
     keys = torch.cat([ok[a:a + c] for a, c in zip(po_h, cnt_h)])

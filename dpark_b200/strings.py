@@ -65,7 +65,7 @@ def reduce_by_key_bytes(splits, key_kind, P, thresholds, op, dev, res):
     mo = shuffle.map_side([rep], [d_vals], P, thresholds, False, sb, row_hash=h, unordered=True)
     rx = shuffle.exchange(mo)
     ok, ov, off, cnt = nv.combine(rx.keys, rx.vals, op, P, rx.seg.contiguous(), rx.part_first, rx.nparts,
-                                  thresholds, sb, row_hash=h)
+                                  thresholds, sb, row_hash=h, rows=rx.rows)
     off_h, cnt_h = off.cpu().tolist(), cnt.cpu().tolist()
     shuffle.check_counts(cnt_h)
     ok_h, ov_h = ok.cpu().numpy(), ov.cpu().numpy()

@@ -166,7 +166,7 @@ def reduce_tokens(text_rdd, split_indices, P, thresholds, op, dev, res, local_on
         mo = shuffle.map_side([rep], [ones], P, thresholds, False, sb, row_hash=h, unordered=True)
         rx = shuffle.exchange(mo)
         ok, ov, poff, cnt = nv.combine(rx.keys, rx.vals, op, P, rx.seg.contiguous(), rx.part_first, rx.nparts,
-                                       thresholds, sb, row_hash=h)
+                                       thresholds, sb, row_hash=h, rows=rx.rows)
     off_h, cnt_h = poff.cpu().tolist(), cnt.cpu().tolist()
     shuffle.check_counts(cnt_h)
     # the distinct words: their bytes are gathered on the device, one small copy back

@@ -47,6 +47,12 @@ enum { DPK_K_I64 = 0, DPK_K_I32 = 1, DPK_K_F64 = 2, DPK_K_U64 = 3, DPK_K_F32 = 4
  * of a bucket in input order (reduceByKey merges them anyway; groupByKey does need the order), which
  * lets the multisplit rank rows with one native shared-memory atomic instead of a warp match. */
 #define DPK_K_UNORDERED 0x100
+/* OR-able into key_kind (not with -1) of dpk_partition / dpk_partition_scatter (values as wide as the keys; not
+ * dpk_partition_scatter_ptrs) and of dpk_combine: rows are PACKED records -- key then value, 16 bytes for 8-byte columns, 8 bytes for 4-byte
+ * ones -- instead of two columns.  dpk_partition*: the output is packed; out_keys receives the records (aligned to the
+ * record size), out_vals is ignored.  dpk_combine: the input is packed; keys points at the records, vals must be
+ * NULL and val_kind still names the value type.  Fewer, longer bucket runs in the multisplits and one load per row. */
+#define DPK_K_PACKED 0x200
 /* value column kinds */
 enum { DPK_V_I64 = 0, DPK_V_F64 = 1, DPK_V_I32 = 2, DPK_V_F32 = 3 };
 /* combiner ops a reduceByKey(func) lowers to (dpark/rdd.py:543-545 builds
