@@ -20,8 +20,9 @@
 //                        that partition's range (CTA-aggregated), write.
 // Common to all: 16-byte slots {key bits, accumulator}; k_tbl_plan computes per-bucket region offsets
 // (1.5 x rows), per-partition output offsets and the first row of every (source, bucket) segment.
-// Accumulators: int64 for integer values (exact while |sum| < 2^63, as the reference's big ints),
-// float64 for float values (the reference adds Python floats).
+// Accumulators: int64 for integer values (exact while |sum| < 2^63, as the reference's big ints; products wrap mod
+// 2^64, so the operator surface refuses a product that could leave int64), float64 for float values (the reference
+// adds Python floats; min / max follow IEEE 754-2019 minimum / maximum, DESIGN.md section 7).
 #include "dpk_common.cuh"
 #include <cooperative_groups.h>
 #include <type_traits>
@@ -88,7 +89,7 @@ template <> struct Acc<int64_t> {
         case DPK_OP_AND: atomicAnd((unsigned long long *)a, (unsigned long long)v); break;
         case DPK_OP_OR: atomicOr((unsigned long long *)a, (unsigned long long)v); break;
         case DPK_OP_XOR: atomicXor((unsigned long long *)a, (unsigned long long)v); break;
-        default: {  // PROD (wrapping, like int64 multiply)
+        default: {  // PROD (wrapping, like int64 multiply: exact whenever the key's final product fits int64)
             unsigned long long old = *(volatile unsigned long long *)a, assumed;
             do {
                 assumed = old;
@@ -120,12 +121,15 @@ template <> struct Acc<double> {
             atomicAdd((double *)a, v);
             return;
         }
+        // MIN / MAX are IEEE 754-2019 minimum / maximum: NaN as soon as either operand is NaN, and -0.0 < +0.0.  Both
+        // are order-free, so an accumulator seeded with the key's first value and one started at +-inf end bitwise
+        // equal on every variant (a NaN already held is kept: no CAS traffic between NaN payloads)
         unsigned long long old = *(volatile unsigned long long *)a, assumed;
         do {
             assumed = old;
             double cur = __longlong_as_double((long long)assumed), nv;
-            if (op == DPK_OP_MIN) nv = v < cur ? v : cur;
-            else if (op == DPK_OP_MAX) nv = v > cur ? v : cur;
+            if (op == DPK_OP_MIN) nv = cur != cur ? cur : (v != v || v < cur || (v == cur && signbit(v))) ? v : cur;
+            else if (op == DPK_OP_MAX) nv = cur != cur ? cur : (v != v || v > cur || (v == cur && !signbit(v))) ? v : cur;
             else nv = cur * v;
             if (__double_as_longlong(nv) == (long long)assumed) break;
             old = atomicCAS((unsigned long long *)a, assumed, (unsigned long long)__double_as_longlong(nv));

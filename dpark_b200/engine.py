@@ -224,7 +224,9 @@ def _run_reduce(splits, P, thr, op, dev):
     res = ShuffleResult(P)
     tensor_in = splits and not isinstance(splits[0], columnar.Columns)
     if tensor_in:
+        from . import join
         kc = [k.to(dev).contiguous() for k, v in splits]
+        join.reject_nan_keys(kc)
         vc = [v.to(dev).contiguous() for k, v in splits]
         parts = shuffle.reduce_by_key(kc, vc, P, op, thr)
         for p, k, v in parts:
@@ -235,6 +237,7 @@ def _run_reduce(splits, P, thr, op, dev):
     if len(vkinds) > 1:
         raise TypeError("reduceByKey values must be all int or all float on the GPU path")
     _check_int_sum_range(splits, vkinds, op)
+    _check_int_prod_range(splits, vkinds, op, lambda logs: _run_reduce(logs, P, thr, "sum", dev))
     if kk in (columnar.KEY_I64, columnar.KEY_F64):
         kdt = np.int64 if kk == columnar.KEY_I64 else np.float64
         kc = [torch.from_numpy(c.keys.astype(kdt, copy=False)).to(dev) for c in splits]
@@ -258,6 +261,32 @@ def _check_int_sum_range(splits, vkinds, op):
         if bound >= 2.0 ** 63:
             raise OverflowError("reduceByKey(add): the values' magnitudes sum to %.3g >= 2^63; int64 accumulation on the "
                                 "GPU path could wrap where the reference's big ints do not" % bound)
+
+
+PROD_LOG2_LIMIT = 63 - 1e-9
+
+
+def _check_int_prod_range(splits, vkinds, op, reduce_sum):
+    """The reference multiplies Python big ints; the device multiplies int64 modulo 2^64.  That is exact whenever a
+    key's final product fits (wrapped intermediates cancel out, and a zero factor makes the exact 0), so only the
+    final magnitude matters: the same reduce, run by `reduce_sum` over log2|v| as float64 sums (a zero gives -inf),
+    must keep every key below 2^63.  Like the sum check this is sufficient and conservative at the boundary: the
+    margin of 1e-9 covers the rounding of the log sums (at most 63 terms of |v| >= 2 can stay below the limit), so a
+    product within a factor 1 - 7e-10 of 2^63, -2^63 included, is refused although it fits."""
+    if vkinds != {columnar.VAL_I64} or op != "prod":
+        return
+    logs = []
+    for c in splits:
+        with np.errstate(divide="ignore"):
+            lv = np.log2(np.abs(c.vals.astype(np.float64)))
+        logs.append(columnar.Columns(c.n, c.key_kind, c.keys, c.key_offsets, columnar.VAL_F64, lv,
+                                     key_objs=c.key_objs))
+    res = reduce_sum(logs)
+    worst = max((max(vals) for _, vals in res.parts if len(vals)), default=float("-inf"))
+    if worst >= PROD_LOG2_LIMIT:
+        raise OverflowError("reduceByKey(mul): a key's integer product has |p| = 2^%.9f, not clearly below 2^63; int64 "
+                            "multiplication on the GPU path would wrap where the reference's big ints do not (the check "
+                            "is conservative at the boundary: [-2] * 63 is refused although -2**63 fits)" % worst)
 
 
 def _run_group(splits, P, thr, dev):

@@ -37,13 +37,19 @@ def device_path_applies(rdds):
     return all(t.dtype in DTYPES and t.dim() == 1 for r in rdds for t in (r.keys, r.vals))
 
 
+def reject_nan_keys(key_columns):
+    """TypeError if a float key column holds a NaN, as the row path's ingest raises (columnar._key_column): CPython
+    hashes NaN by identity, so every NaN row is a key of its own there, while the device would merge equal bits."""
+    for k in key_columns:
+        if k.dtype.is_floating_point and bool(torch.isnan(k).any()):
+            raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
+
+
 def _key_column(rdds, dev):
     """The keys of rdds one after the other on the device, as the row path ingests them; raises TypeError where it
     does (NaN keys, int keys on one input and float keys on another)."""
     sides = [r.keys for r in rdds if r.keys.numel()]
-    for k in sides:
-        if k.dtype.is_floating_point and bool(torch.isnan(k).any()):
-            raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
+    reject_nan_keys(sides)
     kinds = sorted(set("float" if k.dtype.is_floating_point else "int" for k in sides))
     if len(kinds) > 1:
         raise TypeError("mixed key types %s in one shuffle are not supported on the GPU path" % kinds)

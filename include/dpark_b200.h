@@ -219,8 +219,12 @@ int dpk_fused_plan(const int64_t *all_counts, int32_t nranks, int32_t nbuckets, 
  * out_keys/out_vals[out_offsets[j] .. out_offsets[j] + out_counts[j]).  Order
  * inside a partition is unspecified (the reference iterates a dict).
  * Accumulation: I64/I32 values -> int64 (exact while |sum| < 2^63, like the
- * reference's big ints); F64/F32 values -> float64 (the reference adds Python
- * floats); out_vals is 8 bytes per row.  out_keys/out_vals hold n entries.
+ * reference's big ints; products wrap mod 2^64, exact while the final product
+ * fits); F64/F32 values -> float64 (the reference adds Python floats); out_vals
+ * is 8 bytes per row.  out_keys/out_vals hold n entries.
+ * Float MIN / MAX are IEEE 754-2019 minimum / maximum: NaN if any of the key's
+ * values is NaN, otherwise the usual one with -0.0 < +0.0.  The result does not
+ * depend on the merge order, so it is the same on every dpk_set_option setting.
  * n may be an UPPER BOUND of the rows (e.g. the capacity of a receive buffer): every
  * reduce_impl reads only the rows seg_rows describes, so a multi-GPU caller needs no host
  * read of the received row count.

@@ -28,7 +28,7 @@ def _canon(parts):
     return [sorted(([enc(k), enc(v)] for k, v in part), key=json.dumps) for part in parts]
 
 
-REDUCE_CASES = [c for c in SC["cases"] if c["op"] == "reduceByKey" and c["name"] != "mul_small"]
+REDUCE_CASES = [c for c in SC["cases"] if c["op"] == "reduceByKey"]
 
 
 @pytest.mark.parametrize("case", REDUCE_CASES, ids=[c["name"] for c in REDUCE_CASES])

@@ -401,11 +401,60 @@ def test_int_sums_that_could_wrap_are_refused_and_float_zero_keys_are_canonical(
     big = columnar.ingest_pairs([(1, 2 ** 62), (2, 2 ** 62), (1, 5)])
     with pytest.raises(OverflowError):
         engine._check_int_sum_range([big], {columnar.VAL_I64}, "sum")
-    engine._check_int_sum_range([big], {columnar.VAL_I64}, "max")          # only sums can wrap
+    engine._check_int_sum_range([big], {columnar.VAL_I64}, "max")          # min / max cannot wrap (products: below)
     ok = columnar.ingest_pairs([(1, 2 ** 40), (2, -2 ** 40)])
     engine._check_int_sum_range([ok], {columnar.VAL_I64}, "sum")
     c = columnar.ingest_pairs([(-0.0, 1), (0.0, 2)])
     assert np.signbit(c.keys).tolist() == [False, False]
+
+
+def _host_log_sums(logs):
+    """The reduce engine._check_int_prod_range runs, done on the host: per-key sums of the log2 columns."""
+    from dpark_b200 import columnar, engine
+    acc = {}
+    for c in logs:
+        assert c.val_kind == columnar.VAL_F64
+        for k, v in zip(columnar.decode_keys(c.key_kind, c.keys, c.key_offsets, c.key_objs), c.vals.tolist()):
+            acc[k] = acc.get(k, 0.0) + v
+    res = engine.ShuffleResult(1)
+    res.parts[0] = (list(acc), list(acc.values()))
+    return res
+
+
+PROD_GUARD_CASES = [      # (factors of key "k", refused): the other keys of the shuffle have small products
+    ([2] * 63, True),
+    ([-2] * 63, True),                                        # -2**63 fits: refused, the documented conservatism
+    ([2] * 62, False),
+    ([-2] * 62 + [-1], False),
+    ([7, 7, 73, 127, 337, 92737, 649657], True),             # 2**63 - 1: inside the margin below 2^63
+    ([7, 7, 73, 127, 337, 92737, 649657 - 2], False),
+    ([2 ** 50] * 4 + [0], False),                             # a zero among factors totalling 2^200: the product is 0
+    ([2 ** 31 - 1] * 3, True),                                # int32-range factors whose product leaves int64
+    ([2 ** 31 - 1] * 2, False),
+    ([-2 ** 63], True),
+    ([2 ** 62, 1, -1], False),
+]
+
+
+@pytest.mark.parametrize("factors,refused", PROD_GUARD_CASES)
+@pytest.mark.parametrize("key", [5, "k"], ids=["int_key", "str_key"])
+def test_int_products_that_could_wrap_are_refused(factors, refused, key):
+    """engine._check_int_prod_range on ingested columns: refused exactly when log2 of the key's |product| reaches
+    63 - 1e-9, whichever splits its factors arrive in; other ops and float values are never checked."""
+    from dpark_b200 import columnar, engine
+    other = 6 if key == 5 else "j"
+    rows = [(key, f) for f in factors] + [(other, 3), (other, -2 ** 40)]
+    cut = len(rows) // 2
+    splits = [columnar.ingest_pairs(rows[:cut]), columnar.ingest_pairs(rows[cut:])]
+    if refused:
+        with pytest.raises(OverflowError):
+            engine._check_int_prod_range(splits, {columnar.VAL_I64}, "prod", _host_log_sums)
+    else:
+        engine._check_int_prod_range(splits, {columnar.VAL_I64}, "prod", _host_log_sums)
+    for op in ("sum", "min", "max", "and", "or", "xor"):
+        engine._check_int_prod_range(splits, {columnar.VAL_I64}, op, _host_log_sums)
+    floats = [columnar.ingest_pairs([(key, 2.0 ** 40)] * 3)]
+    engine._check_int_prod_range(floats, {columnar.VAL_F64}, "prod", _host_log_sums)
 
 
 def test_merge_part_results_concatenates_partitions_in_order():

@@ -117,8 +117,6 @@ def test_c_restatement_matches_reference(case):
     vs = [np.array([v for _, v in s], dtype=np.float64 if isf else np.int64) for s in splits]
     P = case["P"]
     if case["op"] == "reduceByKey":
-        if case["func"] == "mul":
-            pytest.skip("products overflow int64; covered by the Python restatement")
         got = orc.reduce_by_key(ks, vs, P, OPNAME[case["func"]], case["thresholds"])
         for p in range(P):
             want = {k: dec(v) for k, v in case["parts"][p]}
