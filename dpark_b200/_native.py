@@ -36,7 +36,7 @@ EXPORTS = [
     "dpk_partition_scatter_ptrs", "dpk_copy_segments", "dpk_hash_tuple", "dpk_push_plan", "dpk_push_plan_part", "dpk_pipe_plan", "dpk_fused_plan", "dpk_memcpy_batch",
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
-    "dpk_cogroup_count", "dpk_cogroup_emit",
+    "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
 ]
 
 _lib = None
@@ -103,6 +103,8 @@ def lib():
                                     vp]
         L.dpk_cogroup_count.argtypes = [vp, vp, i64, vp, i32, vp, vp, vp]
         L.dpk_cogroup_emit.argtypes = [vp, vp, vp, i64, i64, vp, i32, i64, vp, vp]
+        L.dpk_topk_lengths.argtypes = [vp, i64, i32, vp, vp]
+        L.dpk_topk_round.argtypes = [vp, vp, i32, i32, vp, i64, i64, vp, i32, i32, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -647,6 +649,31 @@ def cogroup_emit(ids, first, out_off, id_base, vals, n_out):
     out = torch.empty(n_out, dtype=vals.dtype, device=ids.device)
     _check(lib().dpk_cogroup_emit(_ptr(ids), _ptr(first), _ptr(out_off), int(first.numel()), id_base, _ptr(vals),
                                   vals.element_size(), n_out, _ptr(out), _stream()))
+    return out
+
+
+# ---- f4: topByKey selection ----------------------------------------------------------
+TOPK_TILE = 4096      # DPK_TOPK_TILE: candidates per chunk of a round
+TOPK_MAX_N = 512      # DPK_TOPK_MAX_N: the largest top_n the rounds take
+
+
+def topk_lengths(run_starts, top_n):
+    """Per run of candidates (run_starts[G + 1]): its length after one round (dpk_topk_lengths), int64 device [G]."""
+    _need_cuda(run_starts)
+    G = int(run_starts.numel()) - 1
+    out = torch.empty(G, dtype=torch.int64, device=run_starts.device)
+    _check(lib().dpk_topk_lengths(_ptr(run_starts), G, top_n, _ptr(out), _stream()))
+    return out
+
+
+def topk_round(ids, vals, run_starts, n, out_starts, top_n, reverse):
+    """One selection round (dpk_topk_round): candidate i is vals[ids[i]] (ids None: vals[i]) for i < n; out_starts
+    [G + 1] is the exclusive scan of topk_lengths.  Returns the next round's candidates in vals' dtype."""
+    _need_cuda(ids, vals, run_starts, out_starts)
+    out = torch.empty(int(out_starts[-1].item()) if n else 0, dtype=vals.dtype, device=vals.device)
+    _check(lib().dpk_topk_round(_ptr(ids), _ptr(vals), vals.element_size(), int(vals.dtype.is_floating_point),
+                                _ptr(run_starts), int(run_starts.numel()) - 1, n, _ptr(out_starts), top_n,
+                                int(reverse), _ptr(out), _stream()))
     return out
 
 

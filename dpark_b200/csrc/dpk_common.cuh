@@ -276,6 +276,11 @@ DPK_HD PartFn fine_partfn(const PartFn &first, int sb2) {
     return fine;
 }
 
+// a value column of 4- or 8-byte elements moved as raw words (the join / cogroup emits, the topByKey rounds)
+template <int W> struct ValWord;
+template <> struct ValWord<4> { typedef uint32_t T; };
+template <> struct ValWord<8> { typedef uint64_t T; };
+
 // ------------------------------------------------------------- f1: join arithmetic (dpk_join.cu; tests/joincheck.cu
 // runs the same functions on the CPU)
 // A group's id run ids[0 .. len) holds its left rows (ids < nL) before its right rows: the map side is a stable
@@ -331,6 +336,46 @@ DPK_HD void cogroup_split(const int64_t *ids, int64_t s, int64_t len, const int6
 // input's own row number (its values column is indexed from 0, its ids from id_base)
 DPK_HD int64_t cogroup_source(const int64_t *ids, int64_t first, int64_t base, int64_t r, int64_t id_base) {
     return ids[first + r - base] - id_base;
+}
+
+// ------------------------------------------------------------- f4: topByKey arithmetic (dpk_topk.cu; tests/topkcheck.cu
+// runs the same functions on the CPU)
+// The low `width` bytes of a value (int, or IEEE float when is_float) -> a word whose unsigned order is the value's
+// order, complemented for reverse: ints flip the sign bit; floats map -0.0 to +0.0 (they compare equal in Python), then
+// flip the sign bit of positives and every bit of negatives.  NaN has no place in this order; callers keep it out.
+DPK_HD uint64_t topk_order_key(uint64_t bits, int32_t width, bool is_float, bool reverse) {
+    const uint64_t mask = width == 8 ? ~0ull : 0xFFFFFFFFull, sign = width == 8 ? 1ull << 63 : 1ull << 31;
+    bits &= mask;
+    uint64_t k;
+    if (!is_float) {
+        k = bits ^ sign;
+    } else {
+        if (bits == sign) bits = 0;
+        k = (bits & sign) ? (~bits & mask) : (bits | sign);
+    }
+    return reverse ? (~k & mask) : k;
+}
+// A run of L candidates after one round with tile T: its full chunks of T keep top_n each, the rest min(top_n, rest).
+// A run of L <= T is one unit and keeps min(top_n, L), its answer (top_n <= T).
+DPK_HD int64_t topk_next_len(int64_t L, int64_t T, int64_t top_n) {
+    const int64_t rest = L % T;
+    return L / T * top_n + (rest < top_n ? rest : top_n);
+}
+// The unit of run [s, e) that CTA w takes: units are the run's chunks [s + cT, min(e, s + (c + 1)T)), and a CTA takes the
+// units that start in its window of rows [wT, (w + 1)T).  A window holds at most one chunk start of a run.  Returns
+// false when the run has none there; a CTA's units lie in [wT, (w + 2)T).
+DPK_HD bool topk_unit(int64_t s, int64_t e, int64_t w, int64_t T, int64_t *u0, int64_t *u1) {
+    const int64_t w0 = w * T;
+    const int64_t a = s >= w0 ? s : s + (w0 - s + T - 1) / T * T;
+    if (a >= w0 + T || a >= e) return false;
+    *u0 = a;
+    *u1 = e < a + T ? e : a + T;
+    return true;
+}
+// where the unit starting at row u0 of the run that starts at s writes: the run's next-round start out_s plus top_n per
+// full chunk before it
+DPK_HD int64_t topk_unit_out(int64_t s, int64_t u0, int64_t out_s, int64_t T, int64_t top_n) {
+    return out_s + (u0 - s) / T * top_n;
 }
 
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)

@@ -26,10 +26,6 @@ constexpr int JN_THREADS = 256;
 constexpr int JN_ITEMS = 8;
 constexpr int JN_TILE = JN_THREADS * JN_ITEMS;
 
-template <int W> struct ValWord;
-template <> struct ValWord<4> { typedef uint32_t T; };
-template <> struct ValWord<8> { typedef uint64_t T; };
-
 __global__ void __launch_bounds__(256)
 k_join_count(const int64_t *__restrict__ ids, const int64_t *__restrict__ starts, int64_t G, int64_t nL,
              bool keep_left, bool keep_right, int64_t *__restrict__ out_nl, int64_t *__restrict__ out_count) {

@@ -148,15 +148,25 @@ def cogroup_columns(rdds, P, thresholds):
     off = torch.zeros((N, G + 1), dtype=torch.int64, device=dev)
     for t in range(N):      # one 1-D scan per input: torch scans a [N, G] tensor along dim 1 one row per CTA
         torch.cumsum(cnt[t], 0, out=off[t, 1:])
-    # partition p holds the groups [pg[p], pg[p + 1]) and input t's values [rows[t][p], rows[t][p + 1])
+    pg, rows = partition_bounds(gs, part_off, off)
+    cols = [nv.cogroup_emit(ov, first[t], off[t], bounds[t], vals[t], rows[t][-1]) for t in range(N)]
+    return partition_slices(gk.view(keys.dtype), off, cols, pg, rows)
+
+
+def partition_bounds(gs, part_off, off):
+    """Where the partitions of a group-by (group starts gs[G + 1], partition row offsets part_off[P + 1]) lie in its
+    per-group outputs: partition p holds the groups [pg[p], pg[p + 1]) and the rows [rows[t][p], rows[t][p + 1]) of
+    output t, whose group g starts at row off[t, g] (off: [N, G + 1]).  Host lists."""
     pg = torch.searchsorted(gs[:-1], part_off)
     rows = off[:, pg].cpu().tolist()
-    pg = pg.cpu().tolist()
-    cols = [nv.cogroup_emit(ov, first[t], off[t], bounds[t], vals[t], rows[t][-1]) for t in range(N)]
-    if keys.dtype == torch.float64:
-        gk = gk.view(torch.float64)
+    return pg.cpu().tolist(), rows
+
+
+def partition_slices(gk, off, cols, pg, rows):
+    """Per partition (keys[G_p], offsets[N, G_p + 1] starting at 0, (output_0, ...)): views of the group keys, of the
+    per-group output offsets off and of the output columns cols, cut at partition_bounds' (pg, rows)."""
     return [(gk[pg[p]:pg[p + 1]], off[:, pg[p]:pg[p + 1] + 1] - off[:, pg[p]:pg[p] + 1],
-             tuple(cols[t][rows[t][p]:rows[t][p + 1]] for t in range(N))) for p in range(P)]
+             tuple(c[r[p]:r[p + 1]] for c, r in zip(cols, rows))) for p in range(len(pg) - 1)]
 
 
 class ColumnarCoGroupedRDD(RDD):

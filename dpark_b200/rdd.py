@@ -25,6 +25,13 @@ from .errors import DparkUserFatalError  # noqa: F401
 _enumerate = enumerate      # RDD.enumerate shadows the builtin inside the class body
 
 
+def top_values(top_n, order_func, reverse):
+    """topByKey's per-key function: the first top_n values of a stable sort by order_func."""
+    def best(values):
+        return sorted(values, key=order_func, reverse=reverse)[:top_n]
+    return best
+
+
 class Split(object):
     def __init__(self, index):
         self.index = index
@@ -216,6 +223,12 @@ class RDD(object):
     def combineByKey(self, aggregator, splits=None, taskMemory=None, fixSkew=-1, rddconf=None):
         """dpark/rdd.py:511-541.  `splits` is a partition count or a Partitioner; fixSkew > 0 is the sample
         rate for balancing the partitions by hash thresholds instead of hash modulo."""
+        return ShuffledRDD(self, aggregator, self._combine_partitioner(splits, fixSkew), taskMemory, rddconf=rddconf)
+
+    def _combine_partitioner(self, splits, fixSkew):
+        """The partitioner of combineByKey(splits, fixSkew=...) (dpark/rdd.py:511-541): splits defaults to
+        min(defaultMinSplits, partitions); an int becomes a HashPartitioner, with thresholds sampled over self when
+        fixSkew > 0; a Partitioner is taken as it is."""
         if splits is None:
             splits = min(self.ctx.defaultMinSplits, len(self))
         if type(splits) is int:
@@ -223,7 +236,7 @@ class RDD(object):
             if fixSkew > 0 and splits > 1:
                 thresh, splits = self._skew_thresholds(splits, fixSkew)
             splits = HashPartitioner(splits, thresholds=thresh)
-        return ShuffledRDD(self, aggregator, splits, taskMemory, rddconf=rddconf)
+        return splits
 
     def reduceByKey(self, func, numSplits=None, taskMemory=None, fixSkew=-1, rddconf=None):
         """dpark/rdd.py:543-545."""
@@ -326,14 +339,18 @@ class RDD(object):
         The reference keeps a bounded heap per key on both sides of the shuffle (HeapAggregator,
         dpark/dependency.py:164-193) over (order, partition, sequence, value) tuples.  The GPU group-by already
         delivers every key's values in (partition, position) order, so the same answer is a stable sort of that
-        list (Python's sort is stable for reverse=True as well) cut at top_n."""
+        list (Python's sort is stable for reverse=True as well) cut at top_n.
+
+        A numeric ColumnarRDD in a one-process job, with no order_func and top_n <= topk.TOPK_MAX_N, is selected on
+        the device (dpark_b200/topk.py), with the same partitions, keys, values and order as this composition."""
         if top_n <= 0:
             raise AssertionError("top_n must be positive")
-
-        def best(values):
-            return sorted(values, key=order_func, reverse=reverse)[:top_n]
-
-        return self.groupByKey(num_splits, task_memory, fixSkew=fixSkew).mapValue(best)
+        from . import join, topk
+        if order_func is None and type(top_n) is int and top_n <= topk.TOPK_MAX_N and join.device_path_applies([self]):
+            part = self._combine_partitioner(num_splits, fixSkew)
+            if isinstance(part, HashPartitioner):       # other partitioners: the group-by below refuses them
+                return topk.ColumnarTopByKeyRDD(self, part, top_n, reverse)
+        return self.groupByKey(num_splits, task_memory, fixSkew=fixSkew).mapValue(top_values(top_n, order_func, reverse))
 
     def sort(self, key=lambda x: x, reverse=False, numSplits=None, taskMemory=None, rddconf=None):
         """dpark/rdd.py:273-287: a globally sorted RDD.  Range bounds come from the first elements of every

@@ -343,6 +343,25 @@ int dpk_cogroup_count(const int64_t *ids, const int64_t *group_starts, int64_t n
 int dpk_cogroup_emit(const int64_t *ids, const int64_t *first, const int64_t *out_off, int64_t ngroups, int64_t id_base,
                      const void *vals, int32_t val_bytes, int64_t n_out, void *out_vals, dpk_stream_t stream);
 
+/* ---- f4: topByKey (dpark/rdd.py:552-594) of a numeric value column ----------------------------------------------------
+ * Per key the first top_n values of a stable sort of its values (ascending, or descending with reverse != 0), in rounds
+ * over runs of candidates.  Round 1's runs are the group-by's: run_starts = group_starts and candidate i is
+ * vals[ids[i]]; later rounds pass ids = NULL and the previous round's output as vals (candidate i is vals[i]).
+ *   dpk_topk_lengths : out_len[g] = the length of run g after one round (nruns entries): a run of L <= DPK_TOPK_TILE
+ *                      candidates keeps min(top_n, L) -- its answer; a longer one is cut into chunks of DPK_TOPK_TILE
+ *                      from its start and keeps the first top_n of every chunk, floor(L / T) * top_n + min(top_n, L % T).
+ *   dpk_topk_round   : out_starts[nruns + 1] = the exclusive scan of out_len; writes every chunk's (every short run's)
+ *                      first values in order to out_vals.  n = run_starts[nruns].  Equal values keep their candidate
+ *                      order; -0.0 and 0.0 compare equal and keep their bits.  Float values must not be NaN.
+ *                      val_bytes in {4, 8}, val_float != 0 for IEEE values, 1 <= top_n <= DPK_TOPK_MAX_N.
+ * Repeat while the longest run is longer than DPK_TOPK_TILE; then one more round leaves min(top_n, L) values per key. */
+#define DPK_TOPK_TILE 4096
+#define DPK_TOPK_MAX_N 512
+int dpk_topk_lengths(const int64_t *run_starts, int64_t nruns, int32_t top_n, int64_t *out_len, dpk_stream_t stream);
+int dpk_topk_round(const int64_t *ids, const void *vals, int32_t val_bytes, int32_t val_float,
+                   const int64_t *run_starts, int64_t nruns, int64_t n, const int64_t *out_starts, int32_t top_n,
+                   int32_t reverse, void *out_vals, dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
