@@ -37,6 +37,7 @@ EXPORTS = [
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
+    "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit",
 ]
 
 _lib = None
@@ -105,6 +106,9 @@ def lib():
         L.dpk_cogroup_emit.argtypes = [vp, vp, vp, i64, i64, vp, i32, i64, vp, vp]
         L.dpk_topk_lengths.argtypes = [vp, i64, i32, vp, vp]
         L.dpk_topk_round.argtypes = [vp, vp, i32, i32, vp, i64, i64, vp, i32, i32, vp, vp]
+        L.dpk_bcast_build.argtypes = [vp, i64, vp, i64, vp]
+        L.dpk_bcast_probe.argtypes = [vp, i32, i64, vp, i64, vp, vp, vp, vp]
+        L.dpk_bcast_emit.argtypes = [vp, i32, vp, i32, vp, vp, i64, vp, vp, vp, i32, i64, vp, vp, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -675,6 +679,53 @@ def topk_round(ids, vals, run_starts, n, out_starts, top_n, reverse):
                                 _ptr(run_starts), int(run_starts.numel()) - 1, n, _ptr(out_starts), top_n,
                                 int(reverse), _ptr(out), _stream()))
     return out
+
+
+# ---- f5: innerJoin hash table ----------------------------------------------------------
+def bcast_slots(G):
+    """Slots of the innerJoin table of G keys: the least power of two >= max(2, 2 G) (bcast_slots, dpk_common.cuh)."""
+    s = 2
+    while s < 2 * G:
+        s <<= 1
+    return s
+
+
+def bcast_build(group_keys):
+    """The hash table of the distinct normalised keys group_keys[G] (int64 bits): a uint8 device tensor of
+    bcast_slots(G) 16-byte slots (dpk_bcast_build)."""
+    _need_cuda(group_keys)
+    G = int(group_keys.numel())
+    S = bcast_slots(G)
+    table = torch.full((S * 16,), 0xFF, dtype=torch.uint8, device=group_keys.device)
+    _check(lib().dpk_bcast_build(_ptr(group_keys), G, _ptr(table), S, _stream()))
+    return table
+
+
+def bcast_probe(table, keys, group_starts):
+    """Every key of the column `keys` (int32 / int64 / float32 / float64, read in place) looked up in bcast_build's
+    table: (grp int32, count int64) device tensors -- its group or -1, and group_starts[g + 1] - group_starts[g] or 0
+    (dpk_bcast_probe)."""
+    _need_cuda(table, keys, group_starts)
+    n = int(keys.numel())
+    grp = torch.empty(n, dtype=torch.int32, device=keys.device)
+    cnt = torch.empty(n, dtype=torch.int64, device=keys.device)
+    _check(lib().dpk_bcast_probe(_ptr(keys), _KEY_KIND.get(keys.dtype, -1), n, _ptr(table), int(table.numel()) // 16,
+                                 _ptr(group_starts), _ptr(grp), _ptr(cnt), _stream()))
+    return grp, cnt
+
+
+def bcast_emit(keys, lvals, grp, out_off, group_starts, ids, rvals, n_out):
+    """The innerJoin rows (dpk_bcast_emit): (keys, left, right) in the dtypes of keys, lvals and rvals; out_off[n + 1]
+    is the exclusive scan of bcast_probe's counts."""
+    _need_cuda(keys, lvals, grp, out_off, group_starts, ids, rvals)
+    dev = keys.device
+    ok = torch.empty(n_out, dtype=keys.dtype, device=dev)
+    left = torch.empty(n_out, dtype=lvals.dtype, device=dev)
+    right = torch.empty(n_out, dtype=rvals.dtype, device=dev)
+    _check(lib().dpk_bcast_emit(_ptr(keys), keys.element_size(), _ptr(lvals), lvals.element_size(), _ptr(grp),
+                                _ptr(out_off), int(keys.numel()), _ptr(group_starts), _ptr(ids), _ptr(rvals),
+                                rvals.element_size(), n_out, _ptr(ok), _ptr(left), _ptr(right), _stream()))
+    return ok, left, right
 
 
 def set_option(name, value):

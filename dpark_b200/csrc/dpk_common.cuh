@@ -378,6 +378,62 @@ DPK_HD int64_t topk_unit_out(int64_t s, int64_t u0, int64_t out_s, int64_t T, in
     return out_s + (u0 - s) / T * top_n;
 }
 
+// ------------------------------------------------------------- f5: innerJoin hash table (dpk_join.cu; tests/bcastcheck.cu
+// runs the same functions on the CPU)
+// The small side's distinct keys in an open-addressing table of 2^k >= 2 G slots, linear probing.  A slot is 16 bytes so
+// that a probe step is one aligned load; grp = -1 marks an empty slot (the caller fills the table with 0xFF bytes).
+struct __align__(16) BcastSlot {
+    uint64_t key;   // normalised key bits (bcast_key_bits)
+    int32_t grp;    // the key's group, -1 = empty
+    int32_t pad;
+};
+// A key as the table holds it: ints widened to int64, floats widened to float64 with -0.0 spelled 0.0 (Python's dict
+// finds 0.0 under -0.0).  False for NaN, which no dict lookup finds.
+template <typename T> DPK_HD bool bcast_key_bits(T k, uint64_t *kb) {
+    *kb = (uint64_t)(int64_t)k;
+    return true;
+}
+template <> DPK_HD bool bcast_key_bits<double>(double k, uint64_t *kb) {
+    if (k != k) return false;
+    if (k == 0.0) k = 0.0;
+    memcpy(kb, &k, sizeof k);
+    return true;
+}
+template <> DPK_HD bool bcast_key_bits<float>(float k, uint64_t *kb) { return bcast_key_bits<double>((double)k, kb); }
+// slots of a table of G keys: the least power of two >= 2 G (at most half full, so a probe ends at an empty slot)
+DPK_HD uint64_t bcast_slots(int64_t G) {
+    uint64_t s = 2;
+    while (s < 2 * (uint64_t)G) s <<= 1;
+    return s;
+}
+// a key's first slot: all 64 bits mixed (mix64), not portable_hash, which is the identity on small ints and would put
+// keys that differ only above the mask into one slot run
+DPK_HD uint64_t bcast_slot(uint64_t kb, uint64_t mask) { return mix64(kb) & mask; }
+DPK_HD uint64_t bcast_next(uint64_t s, uint64_t mask) { return (s + 1) & mask; }
+// claims the first empty slot of kb's probe sequence for group g; the keys are distinct, so no slot is compared
+DPK_HD void bcast_insert(BcastSlot *table, uint64_t mask, uint64_t kb, int32_t g) {
+    for (uint64_t s = bcast_slot(kb, mask);; s = bcast_next(s, mask)) {
+#ifdef __CUDA_ARCH__
+        const int32_t old = atomicCAS(&table[s].grp, -1, g);
+#else
+        const int32_t old = table[s].grp;
+        if (old == -1) table[s].grp = g;
+#endif
+        if (old == -1) {
+            table[s].key = kb;
+            return;
+        }
+    }
+}
+// kb's group, or -1 when its probe sequence reaches an empty slot first
+DPK_HD int32_t bcast_find(const BcastSlot *table, uint64_t mask, uint64_t kb) {
+    for (uint64_t s = bcast_slot(kb, mask);; s = bcast_next(s, mask)) {
+        const BcastSlot e = table[s];
+        if (e.grp < 0) return -1;
+        if (e.key == kb) return e.grp;
+    }
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

@@ -18,6 +18,16 @@
 //   k_cogroup_emit  : one launch per input, load-balanced over that input's output rows with the tile of k_join_emit;
 //                     output row r of group g is value ids[first[g] + r - out_off[g]] - id_base.
 // Algorithmic bytes of a cogroup emit: per output row 8 (the id) + W read, W written.
+//
+// innerJoin of a big input against a small one (dpark/rdd.py:626-648), no group-by of the big side:
+//   k_bcast_build : one thread per distinct small key; claims a slot of the hash table (BcastSlot, dpk_common.cuh) with
+//                   atomicCAS on its group, linear probing, then stores the key bits.
+//   k_bcast_probe : one thread per big row, the key column read in place; writes the row's group (or -1) and its
+//                   match count.
+//   k_bcast_emit  : load-balanced over OUTPUT rows with the tile of k_join_emit, big rows in the role of groups (a
+//                   missed row occupies no row of any tile).
+// Algorithmic bytes: probe K read, 4 + 8 written per big row; emit per output row K + LW + RW written, K + LW + 8 (the
+// id) + RW read.  Table reads are not credited.
 #include "dpk_common.cuh"
 
 namespace dpk {
@@ -147,6 +157,56 @@ k_cogroup_emit(const int64_t *__restrict__ ids, const int64_t *__restrict__ firs
     }
 }
 
+// innerJoin: the small side's G distinct keys in a hash table (BcastSlot, dpk_common.cuh), every big row probed in place
+__global__ void __launch_bounds__(256)
+k_bcast_build(const int64_t *__restrict__ gkeys, int64_t G, BcastSlot *__restrict__ table, uint64_t mask) {
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    bcast_insert(table, mask, (uint64_t)gkeys[g], (int32_t)g);
+}
+
+template <typename K>
+__global__ void __launch_bounds__(256)
+k_bcast_probe(const K *__restrict__ keys, int64_t n, const BcastSlot *__restrict__ table, uint64_t mask,
+              const int64_t *__restrict__ starts, int32_t *__restrict__ out_grp, int64_t *__restrict__ out_count) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    uint64_t kb;
+    const int32_t g = bcast_key_bits<K>(keys[r], &kb) ? bcast_find(table, mask, kb) : -1;
+    out_grp[r] = g;
+    out_count[r] = g < 0 ? 0 : starts[g + 1] - starts[g];
+}
+
+// the joined rows, load-balanced over output rows with the join's tile; big row r plays the role of a group: its
+// output rows are off[r] .. off[r + 1], one per small row of its key, in ascending small row order (the ids of a
+// group-by run ascend).  Six CTAs per SM: 40 registers; left to itself ptxas picks 32 and spills.
+template <int KW, int LW, int RW>
+__global__ void __launch_bounds__(JN_THREADS, 6)
+k_bcast_emit(const void *__restrict__ keys, const void *__restrict__ lvals, const int32_t *__restrict__ grp,
+             const int64_t *__restrict__ off, int64_t n, const int64_t *__restrict__ starts,
+             const int64_t *__restrict__ ids, const void *__restrict__ rvals, int64_t n_out, void *__restrict__ out_keys,
+             void *__restrict__ out_left, void *__restrict__ out_right) {
+    typedef typename ValWord<KW>::T KT;
+    typedef typename ValWord<LW>::T LT;
+    typedef typename ValWord<RW>::T RT;
+    __shared__ int64_t s_off[JN_TILE + 1];
+    __shared__ int64_t s_g[2];
+    const EmitTile tile = emit_tile(off, n, n_out, s_off, s_g);
+#pragma unroll 2
+    for (int it = 0; it < JN_ITEMS; it++) {
+        const int64_t i = tile.i0 + (int64_t)it * JN_THREADS + threadIdx.x;
+        if (i > tile.i_last) break;
+        int64_t r, base;
+        tile.locate(i, &r, &base);
+        static_cast<KT *>(out_keys)[i] = static_cast<const KT *>(keys)[r];
+        static_cast<LT *>(out_left)[i] = static_cast<const LT *>(lvals)[r];
+        static_cast<RT *>(out_right)[i] = static_cast<const RT *>(rvals)[ids[starts[grp[r]] + i - base]];
+    }
+}
+
+typedef void (*BcastEmitFn)(const void *, const void *, const int32_t *, const int64_t *, int64_t, const int64_t *,
+                            const int64_t *, const void *, int64_t, void *, void *, void *);
+
 }  // namespace dpk
 
 using namespace dpk;
@@ -225,6 +285,76 @@ int dpk_cogroup_emit(const int64_t *ids, const int64_t *first, const int64_t *ou
     else
         DPK_LAUNCH("cogroup_emit", st, k_cogroup_emit<4><<<(unsigned)blocks, JN_THREADS, 0, st>>>(
             ids, first, out_off, ngroups, id_base, vals, n_out, out_vals));
+    return DPK_OK;
+}
+
+int dpk_bcast_build(const int64_t *group_keys, int64_t ngroups, void *table, int64_t nslots, dpk_stream_t stream) {
+    if (ngroups < 0 || ngroups > INT32_MAX || nslots != (int64_t)bcast_slots(ngroups))
+        return fail(DPK_ERR_INVALID, "ngroups=%lld nslots=%lld (want %llu)", (long long)ngroups, (long long)nslots,
+                    (unsigned long long)bcast_slots(ngroups < 0 ? 0 : ngroups));
+    if (ngroups == 0) return DPK_OK;
+    if (!group_keys || !table) return fail(DPK_ERR_INVALID, "NULL pointer");
+    if ((uintptr_t)table % sizeof(BcastSlot)) return fail(DPK_ERR_INVALID, "table not 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t blocks = (ngroups + 255) / 256;
+    DPK_LAUNCH("bcast_build", st, k_bcast_build<<<(unsigned)blocks, 256, 0, st>>>(
+        group_keys, ngroups, static_cast<BcastSlot *>(table), (uint64_t)nslots - 1));
+    return DPK_OK;
+}
+
+int dpk_bcast_probe(const void *keys, int32_t key_kind, int64_t n, const void *table, int64_t nslots,
+                    const int64_t *group_starts, int32_t *out_grp, int64_t *out_count, dpk_stream_t stream) {
+    if (n < 0 || nslots < 2 || (nslots & (nslots - 1)))
+        return fail(DPK_ERR_INVALID, "n=%lld nslots=%lld (a power of two >= 2)", (long long)n, (long long)nslots);
+    if (key_kind != DPK_K_I64 && key_kind != DPK_K_I32 && key_kind != DPK_K_F64 && key_kind != DPK_K_F32)
+        return fail(DPK_ERR_UNSUPPORTED, "key kind %d", (int)key_kind);
+    if (n == 0) return DPK_OK;
+    if (!keys || !table || !group_starts || !out_grp || !out_count) return fail(DPK_ERR_INVALID, "NULL pointer");
+    if ((uintptr_t)table % sizeof(BcastSlot)) return fail(DPK_ERR_INVALID, "table not 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    const BcastSlot *t = static_cast<const BcastSlot *>(table);
+    const uint64_t mask = (uint64_t)nslots - 1;
+    switch (key_kind) {
+    case DPK_K_I64:
+        DPK_LAUNCH("bcast_probe", st, k_bcast_probe<int64_t><<<blocks, 256, 0, st>>>(
+            static_cast<const int64_t *>(keys), n, t, mask, group_starts, out_grp, out_count));
+        break;
+    case DPK_K_I32:
+        DPK_LAUNCH("bcast_probe", st, k_bcast_probe<int32_t><<<blocks, 256, 0, st>>>(
+            static_cast<const int32_t *>(keys), n, t, mask, group_starts, out_grp, out_count));
+        break;
+    case DPK_K_F64:
+        DPK_LAUNCH("bcast_probe", st, k_bcast_probe<double><<<blocks, 256, 0, st>>>(
+            static_cast<const double *>(keys), n, t, mask, group_starts, out_grp, out_count));
+        break;
+    default:
+        DPK_LAUNCH("bcast_probe", st, k_bcast_probe<float><<<blocks, 256, 0, st>>>(
+            static_cast<const float *>(keys), n, t, mask, group_starts, out_grp, out_count));
+    }
+    return DPK_OK;
+}
+
+int dpk_bcast_emit(const void *keys, int32_t key_bytes, const void *lvals, int32_t lval_bytes, const int32_t *grp,
+                   const int64_t *out_off, int64_t n, const int64_t *group_starts, const int64_t *ids,
+                   const void *rvals, int32_t rval_bytes, int64_t n_out, void *out_keys, void *out_left,
+                   void *out_right, dpk_stream_t stream) {
+    if (n < 0 || n_out < 0) return fail(DPK_ERR_INVALID, "n=%lld n_out=%lld", (long long)n, (long long)n_out);
+    if ((key_bytes != 4 && key_bytes != 8) || (lval_bytes != 4 && lval_bytes != 8) ||
+        (rval_bytes != 4 && rval_bytes != 8))
+        return fail(DPK_ERR_UNSUPPORTED, "widths %d / %d / %d bytes (4 or 8)", key_bytes, lval_bytes, rval_bytes);
+    if (n_out == 0) return DPK_OK;
+    if (n == 0) return fail(DPK_ERR_INVALID, "n_out=%lld rows from no big row", (long long)n_out);
+    if (!keys || !lvals || !grp || !out_off || !group_starts || !ids || !rvals || !out_keys || !out_left || !out_right)
+        return fail(DPK_ERR_INVALID, "NULL pointer");
+    static const BcastEmitFn fns[2][2][2] = {
+        {{k_bcast_emit<4, 4, 4>, k_bcast_emit<4, 4, 8>}, {k_bcast_emit<4, 8, 4>, k_bcast_emit<4, 8, 8>}},
+        {{k_bcast_emit<8, 4, 4>, k_bcast_emit<8, 4, 8>}, {k_bcast_emit<8, 8, 4>, k_bcast_emit<8, 8, 8>}}};
+    const BcastEmitFn fn = fns[key_bytes == 8][lval_bytes == 8][rval_bytes == 8];
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t blocks = (n_out + JN_TILE - 1) / JN_TILE;
+    DPK_LAUNCH("bcast_emit", st, fn<<<(unsigned)blocks, JN_THREADS, 0, st>>>(
+        keys, lvals, grp, out_off, n, group_starts, ids, rvals, n_out, out_keys, out_left, out_right));
     return DPK_OK;
 }
 

@@ -17,6 +17,11 @@ The groups come out partition by partition in the order of the group-by of the t
 groupWith / cogroup of N numeric ColumnarRDDs (CoGroupedRDD, a group-by of the tagged union) and groupByKey of one
 (N = 1) take the same CSR without a cross product: dpk_cogroup_count splits every key's id run at the inputs' id
 boundaries, and dpk_cogroup_emit gathers each input's value runs, load-balanced like the join's emit.
+
+innerJoin (dpark/rdd.py:626-648) keeps the big side where it lies: no group-by, no shuffle, its splits and row order.
+Only the small side is grouped (P = 1, with row ids, so each key's ids ascend: small.collect() order); its distinct
+keys go into a device hash table (dpk_bcast_build), every big row is probed in place (dpk_bcast_probe: its group and
+match count), and after one scan of the counts dpk_bcast_emit writes the rows, load-balanced like the join's emit.
 """
 import torch
 
@@ -122,6 +127,74 @@ class ColumnarJoinedRDD(RDD):
         if rvalid is not None:
             rs = [y if ok else None for y, ok in zip(rs, rvalid.cpu().tolist())]
         return zip(keys.cpu().tolist(), zip(ls, rs))
+
+
+def inner_join_applies(big, small):
+    """True when big.innerJoin(small) runs on the device: device_path_applies, and not int keys on one side with float
+    keys on the other (both non-empty; Python's 1 == 1.0 is not the device's equality)."""
+    if not device_path_applies([big, small]):
+        return False
+    sides = [r.keys for r in (big, small) if r.keys.numel()]
+    return len(set(k.dtype.is_floating_point for k in sides)) <= 1
+
+
+def inner_join_columns(big, small):
+    """big.innerJoin(small) of two ColumnarRDDs: a list of tuples (keys, left, right) of CUDA tensors, one per split of
+    big, in big's key and value dtypes and small's value dtype."""
+    from .engine import _device
+    dev = _device()
+    keys, lvals = big.keys.to(dev).contiguous(), big.vals.to(dev).contiguous()
+    rvals = small.vals.to(dev).contiguous()
+    split_rows = [sp.begin for sp in big.splits] + [big.splits[-1].end]
+    # the small keys as the dict holds them: int -> int64, float -> float64 with 0.0 for -0.0; NaN keys find nothing
+    sk = small.keys.to(dev)
+    ids = torch.arange(sk.numel(), dtype=torch.int64, device=dev)
+    if sk.dtype.is_floating_point:
+        sk = sk.to(torch.float64) + 0.0
+        keep = ~torch.isnan(sk)
+        sk, ids = sk[keep], ids[keep]
+    else:
+        sk = sk.to(torch.int64)
+    if keys.numel() == 0 or sk.numel() == 0:
+        empty = (keys[:0], lvals[:0], rvals[:0])
+        return [empty] * len(big.splits)
+    gk, gs, ov, _ = grouping.group_row_ids([sk], [ids], 1, None)
+    table = nv.bcast_build(gk)
+    grp, cnt = nv.bcast_probe(table, keys, gs)
+    off = torch.zeros(keys.numel() + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(cnt, 0, out=off[1:])
+    rows = off[split_rows].cpu().tolist()
+    cols = nv.bcast_emit(keys, lvals, grp, off, gs, ov, rvals, rows[-1])
+    return [tuple(c[rows[s]:rows[s + 1]] for c in cols) for s in range(len(big.splits))]
+
+
+class ColumnarInnerJoinedRDD(RDD):
+    """The result of big.innerJoin(small) of two numeric ColumnarRDDs in a one-process job: the rows RDD.innerJoin's
+    flatMap yields, computed on the GPU the first time a partition is asked for and kept.  Like the flatMap it has
+    big's splits and no partitioner."""
+
+    def __init__(self, big, small):
+        RDD.__init__(self, big.ctx)
+        self.big, self.small = big, small
+        self._splits = [Split(i) for i in range(len(big.splits))]
+        self._result = None
+
+    def parents(self):
+        return [self.big, self.small]
+
+    def _materialize(self):
+        if self._result is None:
+            self._result = inner_join_columns(self.big, self.small)
+        return self._result
+
+    def columns(self, split):
+        """Extension: partition `split` (the rows of big's split `split`) as CUDA tensors (keys, left, right): keys in
+        big's key dtype with their own bits, left in big's value dtype, right in small's value dtype."""
+        return self._materialize()[split.index]
+
+    def compute(self, split):
+        keys, left, right = self.columns(split)
+        return zip(keys.cpu().tolist(), zip(left.cpu().tolist(), right.cpu().tolist()))
 
 
 def cogroup_columns(rdds, P, thresholds):

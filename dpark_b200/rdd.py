@@ -395,7 +395,13 @@ class RDD(object):
         return both.mapValue(pick)
 
     def innerJoin(self, smallRdd):
-        """dpark/rdd.py:626-647: join against a small RDD held as a dict on the host (no shuffle)."""
+        """dpark/rdd.py:626-647: join against a small RDD held as a dict on the host (no shuffle).
+
+        Two numeric ColumnarRDDs in a one-process job, with int keys on both sides or float keys on both (or an empty
+        side), are joined on the device (dpark_b200/join.py): the same splits, rows and order as this composition."""
+        from . import join
+        if join.inner_join_applies(self, smallRdd):
+            return join.ColumnarInnerJoinedRDD(self, smallRdd)
         import collections
         table = collections.defaultdict(list)
         for k, v in smallRdd.collect():

@@ -343,6 +343,26 @@ int dpk_cogroup_count(const int64_t *ids, const int64_t *group_starts, int64_t n
 int dpk_cogroup_emit(const int64_t *ids, const int64_t *first, const int64_t *out_off, int64_t ngroups, int64_t id_base,
                      const void *vals, int32_t val_bytes, int64_t n_out, void *out_vals, dpk_stream_t stream);
 
+/* ---- f5: innerJoin (dpark/rdd.py:626-648) of a big column against a small one --------------------------------------
+ * The small side's distinct keys go into a hash table; every big row is probed in place and expands to one output row
+ * per small row of its key.  Keys are compared as normalised bits: ints widened to int64, floats widened to float64
+ * with -0.0 spelled 0.0; a NaN key matches nothing.
+ *   dpk_bcast_build : group_keys[ngroups] = the small side's distinct normalised keys (int64 bits, e.g. a group-by's
+ *                     group keys), ngroups <= INT32_MAX; table = nslots 16-byte slots, 16-byte aligned, every byte
+ *                     0xFF on entry; nslots = the least power of two >= max(2, 2 * ngroups).
+ *   dpk_bcast_probe : keys[n] of kind DPK_K_I64 / I32 / F64 / F32, read in place.  out_grp[r] (int32) = the group of
+ *                     key r or -1, out_count[r] (int64) = group_starts[g + 1] - group_starts[g], 0 on a miss.
+ *   dpk_bcast_emit  : out_off[n + 1] = the exclusive scan of out_count (n_out = out_off[n]).  Output row out_off[r] + j
+ *                     of big row r: out_keys = keys[r] (its own bits), out_left = lvals[r], out_right =
+ *                     rvals[ids[group_starts[grp[r]] + j]].  key_bytes / lval_bytes / rval_bytes in {4, 8}. */
+int dpk_bcast_build(const int64_t *group_keys, int64_t ngroups, void *table, int64_t nslots, dpk_stream_t stream);
+int dpk_bcast_probe(const void *keys, int32_t key_kind, int64_t n, const void *table, int64_t nslots,
+                    const int64_t *group_starts, int32_t *out_grp, int64_t *out_count, dpk_stream_t stream);
+int dpk_bcast_emit(const void *keys, int32_t key_bytes, const void *lvals, int32_t lval_bytes, const int32_t *grp,
+                   const int64_t *out_off, int64_t n, const int64_t *group_starts, const int64_t *ids,
+                   const void *rvals, int32_t rval_bytes, int64_t n_out, void *out_keys, void *out_left,
+                   void *out_right, dpk_stream_t stream);
+
 /* ---- f4: topByKey (dpark/rdd.py:552-594) of a numeric value column ----------------------------------------------------
  * Per key the first top_n values of a stable sort of its values (ascending, or descending with reverse != 0), in rounds
  * over runs of candidates.  Round 1's runs are the group-by's: run_starts = group_starts and candidate i is
