@@ -37,7 +37,7 @@ EXPORTS = [
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
-    "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit",
+    "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
 ]
 
 _lib = None
@@ -109,6 +109,9 @@ def lib():
         L.dpk_bcast_build.argtypes = [vp, i64, vp, i64, vp]
         L.dpk_bcast_probe.argtypes = [vp, i32, i64, vp, i64, vp, vp, vp, vp]
         L.dpk_bcast_emit.argtypes = [vp, i32, vp, i32, vp, vp, i64, vp, vp, vp, i32, i64, vp, vp, vp, vp]
+        L.dpk_sort_keys.argtypes = [vp, i32, vp, i32, i64, i32, vp, vp, vp, vp, vp]
+        L.dpk_sort_cuts.argtypes = [vp, vp, vp, i32, i64, vp, i32, vp, i32, i32, vp, vp]
+        L.dpk_sort_gather.argtypes = [vp, i32, vp, i32, vp, i64, vp, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -726,6 +729,44 @@ def bcast_emit(keys, lvals, grp, out_off, group_starts, ids, rvals, n_out):
                                 _ptr(out_off), int(keys.numel()), _ptr(group_starts), _ptr(ids), _ptr(rvals),
                                 rvals.element_size(), n_out, _ptr(ok), _ptr(left), _ptr(right), _stream()))
     return ok, left, right
+
+
+# ---- f6: sort ------------------------------------------------------------------------
+def sort_keys(col0, col1, reverse):
+    """The order words of one or two order columns (dpk_sort_keys): (w0, w1 | None, ids, nan_flag) int64 / int32 device
+    tensors; w0[i] / w1[i] are row i's words, ids = 0..n-1, nan_flag[0] = 1 when an order column holds a NaN."""
+    _need_cuda(col0, col1)
+    n, dev = int(col0.numel()), col0.device
+    w0 = torch.empty(n, dtype=torch.int64, device=dev)
+    w1 = torch.empty(n, dtype=torch.int64, device=dev) if col1 is not None else None
+    ids = torch.empty(n, dtype=torch.int64, device=dev)
+    flag = torch.zeros(1, dtype=torch.int32, device=dev)
+    _check(lib().dpk_sort_keys(_ptr(col0), _KEY_KIND.get(col0.dtype, -1), _ptr(col1),
+                               -1 if col1 is None else _KEY_KIND.get(col1.dtype, -1), n, int(reverse), _ptr(w0), _ptr(w1),
+                               _ptr(ids), _ptr(flag), _stream()))
+    return w0, w1, ids, flag
+
+
+def sort_cuts(sorted_w0, ids, vals, bounds0, dtype0, bounds1, reverse):
+    """The partition starts of the sorted rows (dpk_sort_cuts): int64 device [nbounds + 2], 0 first and n last.  bounds0 /
+    bounds1: int64 device tensors of the bounds' widened bits (RangePartitioner.keys order), dtype0 the type of the first
+    order column; bounds1 (None unless the order is (k, v)) pairs with the value column vals."""
+    _need_cuda(sorted_w0, ids, vals, bounds0, bounds1)
+    nb = int(bounds0.numel())
+    out = torch.empty(nb + 2, dtype=torch.int64, device=sorted_w0.device)
+    _check(lib().dpk_sort_cuts(_ptr(sorted_w0), _ptr(ids), _ptr(vals), _KEY_KIND.get(vals.dtype, -1),
+                               int(sorted_w0.numel()), _ptr(bounds0), _KEY_KIND.get(dtype0, -1), _ptr(bounds1), nb,
+                               int(reverse), _ptr(out), _stream()))
+    return out
+
+
+def sort_gather(keys, vals, ids):
+    """keys[ids], vals[ids] in their own dtypes, bits preserved (dpk_sort_gather)."""
+    _need_cuda(keys, vals, ids)
+    ok, ov = torch.empty_like(keys), torch.empty_like(vals)
+    _check(lib().dpk_sort_gather(_ptr(keys), keys.element_size(), _ptr(vals), vals.element_size(), _ptr(ids),
+                                 int(ids.numel()), _ptr(ok), _ptr(ov), _stream()))
+    return ok, ov
 
 
 def set_option(name, value):

@@ -434,6 +434,50 @@ DPK_HD int32_t bcast_find(const BcastSlot *table, uint64_t mask, uint64_t kb) {
     }
 }
 
+// ------------------------------------------------------------- f6: sort arithmetic (dpk_sort.cu; tests/sortcheck.cu runs the
+// same functions on the CPU)
+// Element i of a column of kind DPK_K_I32 / I64 / F32 / F64 widened to 64 bits: ints to int64, floats to float64 (both
+// exact and order-keeping, and the values Python sees), returned as the bit pattern.
+DPK_HD bool sort_kind_float(int32_t kind) { return kind == DPK_K_F32 || kind == DPK_K_F64; }
+DPK_HD uint64_t sort_wide_bits(const void *col, int32_t kind, int64_t i) {
+    if (kind == DPK_K_I32) return (uint64_t)(int64_t) static_cast<const int32_t *>(col)[i];
+    if (kind == DPK_K_F32) {
+        const double d = (double)static_cast<const float *>(col)[i];
+        uint64_t b;
+        memcpy(&b, &d, sizeof b);
+        return b;
+    }
+    return static_cast<const uint64_t *>(col)[i];
+}
+DPK_HD bool sort_is_nan(uint64_t wide_bits) { return (wide_bits & ~(1ull << 63)) > 0x7FF0000000000000ull; }
+// The 64-bit order word of a widened value: topk_order_key at width 8, complemented for reverse.
+DPK_HD uint64_t sort_word(uint64_t wide_bits, bool is_float, bool reverse) {
+    return topk_order_key(wide_bits, 8, is_float, reverse);
+}
+// Lexicographic order of rows of nw (1 or 2) order words: -1, 0 or 1.
+DPK_HD int sort_cmp(uint64_t a0, uint64_t a1, uint64_t b0, uint64_t b1, int32_t nw) {
+    if (a0 != b0) return a0 < b0 ? -1 : 1;
+    if (nw == 1 || a1 == b1) return 0;
+    return a1 < b1 ? -1 : 1;
+}
+// Partition j >= 1 of L + 1 starts at the bound sorted_bounds[sort_cut_bound(j, L, reverse)]: getPartition is the number
+// of bounds <= key ascending, the number of bounds > key for reverse.
+DPK_HD int32_t sort_cut_bound(int32_t j, int32_t L, bool reverse) { return reverse ? L - j : j - 1; }
+// Where that partition starts among n rows sorted by their order words: the first row >= the bound's words (lower
+// bound; ascending), or > them (upper bound; reverse, whose words are complemented).  Row i's first word is w0[i]; with
+// nw = 2 its second word is computed from vals[ids[i]] (the value column of kind vkind).
+DPK_HD int64_t sort_cut(const uint64_t *w0, const int64_t *ids, const void *vals, int32_t vkind, int64_t n, uint64_t t0,
+                        uint64_t t1, int32_t nw, bool reverse) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        const uint64_t m1 = nw == 2 ? sort_word(sort_wide_bits(vals, vkind, ids[mid]), sort_kind_float(vkind), reverse) : 0;
+        const int c = sort_cmp(w0[mid], m1, t0, t1, nw);
+        if (reverse ? c <= 0 : c < 0) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

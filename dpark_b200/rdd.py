@@ -32,6 +32,12 @@ def top_values(top_n, order_func, reverse):
     return best
 
 
+def range_bounds(samples, numSplits, reverse):
+    """RDD.sort's range bounds (dpark/rdd.py:273-287) from its samples (the first rows of every split, mapped by the
+    key): every 10th of the sorted samples, from the 6th on, at most numSplits - 1 of them."""
+    return sorted(samples, reverse=reverse)[5::10][:numSplits - 1]
+
+
 class Split(object):
     def __init__(self, index):
         self.index = index
@@ -354,10 +360,19 @@ class RDD(object):
 
     def sort(self, key=lambda x: x, reverse=False, numSplits=None, taskMemory=None, rddconf=None):
         """dpark/rdd.py:273-287: a globally sorted RDD.  Range bounds come from the first elements of every
-        partition exactly as in the reference (every 10th of the sorted sample, offset 5); each element is routed to
-        its range on the host (RangePartitioner) and the shuffle runs on the GPU keyed by the RANGE INDEX --
-        portable_hash(i) % P == i for 0 <= i < P, so HashPartitioner(P) reproduces the reference's layout -- then
-        every partition is sorted."""
+        partition exactly as in the reference (range_bounds); each element is routed to its range on the host
+        (RangePartitioner) and the shuffle runs on the GPU keyed by the RANGE INDEX -- portable_hash(i) % P == i for
+        0 <= i < P, so HashPartitioner(P) reproduces the reference's layout -- then every partition is sorted.
+
+        A numeric ColumnarRDD in a one-process job, sorted by the identity, x[0] or x[1], is sorted on the device
+        (dpark_b200/sorting.py), with the same partitions and rows in the same order as this composition."""
+        from . import sorting
+        if sorting.device_sort_applies(self, key):
+            return sorting.ColumnarSortedRDD(self, key, reverse, numSplits, taskMemory, rddconf)
+        return self._sort_rows(key, reverse, numSplits, taskMemory, rddconf)
+
+    def _sort_rows(self, key, reverse, numSplits, taskMemory, rddconf):
+        """RDD.sort's composition over the rows."""
         if not len(self):
             return self
         if len(self) == 1:
@@ -366,7 +381,7 @@ class RDD(object):
             numSplits = min(self.ctx.defaultMinSplits, len(self))
         n = max(numSplits * 10 // len(self), 1)
         samples = self.mapPartitions(lambda it: itertools.islice(it, n)).map(key).collect()
-        ranges = RangePartitioner(sorted(samples, reverse=reverse)[5::10][:numSplits - 1], reverse=reverse)
+        ranges = RangePartitioner(range_bounds(samples, numSplits, reverse), reverse=reverse)
         routed = self.map(lambda x: (ranges.getPartition(key(x)), x)) \
                      .groupByKey(ranges.numPartitions, taskMemory, rddconf=rddconf)
         return routed.flatMap(lambda kv: kv[1]).mapPartitions(lambda it: sorted(it, key=key, reverse=reverse))

@@ -382,6 +382,29 @@ int dpk_topk_round(const int64_t *ids, const void *vals, int32_t val_bytes, int3
                    const int64_t *run_starts, int64_t nruns, int64_t n, const int64_t *out_starts, int32_t top_n,
                    int32_t reverse, void *out_vals, dpk_stream_t stream);
 
+/* ---- f6: sort (dpark/rdd.py:273-287) of a numeric (k, v) column pair --------------------------------------------------
+ * One global stable sort by order words, then the range partitions as slices of it.  Columns are read in place, of kind
+ * DPK_K_I64 / I32 / F64 / F32.  A value is widened to 64 bits (ints to int64, floats to float64) and its order word is
+ * topk_order_key of those bits at width 8, complemented when reverse != 0: unsigned order of the words is the values'
+ * order (descending with reverse), -0.0 and 0.0 get one word.  NaN has no word.
+ *   dpk_sort_keys   : col0 (kind0) is the first order column, col1 (kind1) the second one or NULL.  out_w0[i] / out_w1[i]
+ *                     = the order words of row i (int64 bits), out_ids[i] = i; *nan_flag (device int32) is set to 1 if an
+ *                     order column holds a NaN (the caller clears it).  n < 2^31.
+ *   dpk_sort_cuts   : sorted_w0[n] = the first order words after the sort, ids[n] the row ids in that order.  bounds0[nbounds]
+ *                     = the range bounds' first order values ascending (RangePartitioner.keys), widened bits of kind0's
+ *                     type; bounds1 = their second values (the (k, v) order; NULL otherwise), whose rows' second words are
+ *                     recomputed from vals[ids[i]] of val_kind.  out_starts[nbounds + 2]: 0, the first row of every
+ *                     partition j = 1 .. nbounds, n.  Ascending, partition j starts at the first row whose words are >=
+ *                     bound j - 1's; reverse, at the first row whose words are > bound nbounds - j's.
+ *   dpk_sort_gather : out_keys[i] = keys[ids[i]], out_vals[i] = vals[ids[i]], key_bytes / val_bytes in {4, 8}. */
+int dpk_sort_keys(const void *col0, int32_t kind0, const void *col1, int32_t kind1, int64_t n, int32_t reverse,
+                  int64_t *out_w0, int64_t *out_w1, int64_t *out_ids, int32_t *nan_flag, dpk_stream_t stream);
+int dpk_sort_cuts(const int64_t *sorted_w0, const int64_t *ids, const void *vals, int32_t val_kind, int64_t n,
+                  const int64_t *bounds0, int32_t kind0, const int64_t *bounds1, int32_t nbounds, int32_t reverse,
+                  int64_t *out_starts, dpk_stream_t stream);
+int dpk_sort_gather(const void *keys, int32_t key_bytes, const void *vals, int32_t val_bytes, const int64_t *ids,
+                    int64_t n, void *out_keys, void *out_vals, dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
