@@ -38,6 +38,7 @@ EXPORTS = [
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
     "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
+    "dpk_tdigest_heads", "dpk_tdigest_build", "dpk_tdigest_merge",
 ]
 
 _lib = None
@@ -112,6 +113,9 @@ def lib():
         L.dpk_sort_keys.argtypes = [vp, i32, vp, i32, i64, i32, vp, vp, vp, vp, vp]
         L.dpk_sort_cuts.argtypes = [vp, vp, vp, i32, i64, vp, i32, vp, i32, i32, vp, vp]
         L.dpk_sort_gather.argtypes = [vp, i32, vp, i32, vp, i64, vp, vp, vp]
+        L.dpk_tdigest_heads.argtypes = [vp, i64, vp, i64, i64, vp, vp]
+        L.dpk_tdigest_build.argtypes = [vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp]
+        L.dpk_tdigest_merge.argtypes = [vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i32, vp, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -767,6 +771,51 @@ def sort_gather(keys, vals, ids):
     _check(lib().dpk_sort_gather(_ptr(keys), keys.element_size(), _ptr(vals), vals.element_size(), _ptr(ids),
                                  int(ids.numel()), _ptr(ok), _ptr(ov), _stream()))
     return ok, ov
+
+
+# ---- f7: percentilesByKey digests ---------------------------------------------------------
+TD_CAP = 209          # TD_CAP: the add path folds when buffered values + centroids reach it; a digest's most centroids
+
+
+def tdigest_heads(ids, group_starts, per):
+    """uint8 device [n]: 1 at every row of the group-by's ids that starts a (key, split) segment, split = id // per
+    (dpk_tdigest_heads)."""
+    _need_cuda(ids, group_starts)
+    n = int(ids.numel())
+    head = torch.zeros(n, dtype=torch.uint8, device=ids.device)
+    _check(lib().dpk_tdigest_heads(_ptr(ids), n, _ptr(group_starts), int(group_starts.numel()) - 1, per, _ptr(head),
+                                   _stream()))
+    return head
+
+
+def tdigest_build(ids, vals, seg_starts, seg_off, flag):
+    """Every segment's t-digest (dpk_tdigest_build): (means, weights, counts, lohi) device tensors -- segment s holds
+    counts[s] centroids at means / weights[seg_off[s]:], lohi[2 s : 2 s + 2] its extreme means.  Sets flag[0] when the
+    composition must stand."""
+    _need_cuda(ids, vals, seg_starts, seg_off, flag)
+    S, dev = int(seg_starts.numel()) - 1, ids.device
+    cm = torch.empty(int(ids.numel()), dtype=torch.float64, device=dev)
+    cw = torch.empty_like(cm)
+    cnt = torch.empty(S, dtype=torch.int32, device=dev)
+    lohi = torch.empty(2 * S, dtype=torch.float64, device=dev)
+    work = torch.empty(S + 2, dtype=torch.int64, device=dev)
+    _check(lib().dpk_tdigest_build(_ptr(ids), _ptr(vals), _KEY_KIND.get(vals.dtype, -1), _ptr(seg_starts),
+                                   _ptr(seg_off), S, _ptr(cm), _ptr(cw), _ptr(cnt), _ptr(lohi), _ptr(work), _ptr(flag),
+                                   _stream()))
+    return cm, cw, cnt, lohi
+
+
+def tdigest_merge(group_starts, seg_starts, seg_off, digests, qs, flag):
+    """quantile(q) of every key's merged digest for every q of the float64 device tensor qs (dpk_tdigest_merge):
+    float64 device [G, len(qs)].  digests: tdigest_build's result.  Sets flag[0] when the composition must stand."""
+    cm, cw, cnt, lohi = digests
+    _need_cuda(group_starts, seg_starts, seg_off, cm, cw, cnt, lohi, qs, flag)
+    G, nq = int(group_starts.numel()) - 1, int(qs.numel())
+    out = torch.empty((G, nq), dtype=torch.float64, device=group_starts.device)
+    _check(lib().dpk_tdigest_merge(_ptr(group_starts), G, _ptr(seg_starts), _ptr(seg_off), int(seg_starts.numel()) - 1,
+                                   _ptr(cnt), _ptr(lohi), _ptr(cm), _ptr(cw), _ptr(qs), nq, _ptr(out), _ptr(flag),
+                                   _stream()))
+    return out
 
 
 def set_option(name, value):

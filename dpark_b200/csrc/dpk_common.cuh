@@ -478,6 +478,176 @@ DPK_HD int64_t sort_cut(const uint64_t *w0, const int64_t *ids, const void *vals
     return lo;
 }
 
+// ------------------------------------------------------------- f7: t-digest arithmetic (dpk_tdigest.cu; tests/tdigestcheck.cu
+// runs the same functions on the CPU).  dpark_b200/quantiles.py operation for operation: every sum, product and
+// quotient is rounded on its own in Python's order (the __d*_rn intrinsics are never contracted into an FMA), and min /
+// max are Python's, which keep the first argument unless the second compares strictly below / above it.
+constexpr int TD_CAP = 209;            // capacity - 1 = 2 * ceil(100) + 10 - 1: a full buffer plus the centroids
+constexpr int TD_STAGE = 2 * TD_CAP;   // the longest fold the kernels stage; a longer one keeps the composition
+constexpr double TD_COMPRESSION = 100.0;
+DPK_HD double td_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+DPK_HD double td_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+DPK_HD double td_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+DPK_HD double td_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+DPK_HD double td_min(double a, double b) { return b < a ? b : a; }
+DPK_HD double td_max(double a, double b) { return b > a ? b : a; }
+// Element i of a value column of kind DPK_K_I32 / I64 / F32 / F64 as Python's float(x): ints round to nearest.
+DPK_HD double td_value(const void *col, int32_t kind, int64_t i) {
+    if (kind == DPK_K_I32) return (double)static_cast<const int32_t *>(col)[i];
+    if (kind == DPK_K_I64) return (double)static_cast<const int64_t *>(col)[i];
+    if (kind == DPK_K_F32) return (double)static_cast<const float *>(col)[i];
+    return static_cast<const double *>(col)[i];
+}
+// zz <= q * (1 - q) with q = a / total, the quotient rounded as Python rounds it (0 <= a <= total; r = 1 / total).  The
+// product with the reciprocal lies within 3 ulp of 1 of the quotient, so q * (1 - q) moves by less than 1e-15; outside a
+// band of 4e-15 around zz the answer is settled without the division.
+DPK_HD bool td_within(double zz, double a, double total, double r) {
+    const double qa = td_mul(a, r), d = td_sub(zz, td_mul(qa, td_sub(1.0, qa)));
+    if (d > 4e-15) return false;
+    if (d < -4e-15) return true;
+    const double q = td_div(a, total);
+    return zz <= td_mul(q, td_sub(1.0, q));
+}
+// _fold's scale test: does the next entry (weight w) join the open centroid (weight W), `done` the weight before it?
+DPK_HD bool td_fuses(double W, double w, double done, double total, double norm, double r) {
+    const double fused = td_add(W, w), z = td_mul(fused, norm), zz = td_mul(z, z);
+    return td_within(zz, done, total, r) && td_within(zz, td_add(done, fused), total, r);
+}
+DPK_HD double td_norm(double total) { return td_div(TD_COMPRESSION, td_mul(M_PI, total)); }
+// out_m[-1] + (ms[i] - out_m[-1]) * ws[i] / out_w[-1], W the centroid's weight with w already added
+DPK_HD double td_mean_step(double m, double x, double w, double W) {
+    return td_add(m, td_div(td_mul(td_sub(x, m), w), W));
+}
+// A fold's first pass, over its n entries' weights in merged order: which entries open a centroid.  The scale test reads
+// weights only, so the means follow per centroid (td_centroid).  cstart[c] = the first entry of centroid c, cstart[count]
+// = n; returns the count.
+DPK_HD int td_fold_decide(const double *xw, int n, double total, int16_t *cstart) {
+    if (n == 0) return 0;
+    const double norm = td_norm(total), r = td_div(1.0, total);
+    double W = xw[0], done = 0.0;
+    int c = 0;
+    cstart[0] = 0;
+    for (int i = 1; i < n; i++) {
+        if (td_fuses(W, xw[i], done, total, norm, r)) {
+            W = td_add(W, xw[i]);
+        } else {
+            done = td_add(done, W);
+            W = xw[i];
+            cstart[++c] = (int16_t)i;
+        }
+    }
+    cstart[c + 1] = (int16_t)n;
+    return c + 1;
+}
+// The mean and weight of the centroid made of entries [s, e) (xw == NULL: every weight 1)
+DPK_HD void td_centroid(const double *xm, const double *xw, int s, int e, double *m, double *W) {
+    double mm = xm[s], ww = xw ? xw[s] : 1.0;
+    for (int i = s + 1; i < e; i++) {
+        const double w = xw ? xw[i] : 1.0;
+        ww = td_add(ww, w);
+        mm = td_mean_step(mm, xm[i], w, ww);
+    }
+    *m = mm;
+    *W = ww;
+}
+// A centroid mean the next fold can take: not NaN and not below its predecessor.  Means of finite values never fall
+// (each is a rounded point between its first and last entry); a NaN (inf - inf) or an overflowed x - m has no answer
+// but the composition's.
+DPK_HD bool td_mean_ok(double m, const double *prev) { return prev ? m >= *prev : m == m; }
+// The whole fold in one pass (the two passes above interleaved) for one thread: centroids to (om, ow), which may alias
+// (xm, xw) since centroid c is written after entry c is read.  *bad is set as by td_mean_ok.  Returns the count.
+DPK_HD int td_fold_serial(const double *xm, const double *xw, int n, double total, double *om, double *ow, bool *bad) {
+    if (n == 0) return 0;
+    const double norm = td_norm(total), r = td_div(1.0, total);
+    double m = xm[0], W = xw ? xw[0] : 1.0, done = 0.0, prev = 0.0;
+    int c = 0;
+    for (int i = 1; i < n; i++) {
+        const double w = xw ? xw[i] : 1.0, x = xm[i];
+        if (td_fuses(W, w, done, total, norm, r)) {
+            W = td_add(W, w);
+            m = td_mean_step(m, x, w, W);
+        } else {
+            *bad |= !td_mean_ok(m, c ? &prev : nullptr);
+            om[c] = m; ow[c] = W; prev = m; c++;
+            done = td_add(done, W);
+            m = x; W = w;
+        }
+    }
+    *bad |= !td_mean_ok(m, c ? &prev : nullptr);
+    om[c] = m; ow[c] = W;
+    return c + 1;
+}
+// Stable insertion sort of a short buffer by value (-0.0 and 0.0 compare equal and keep their order)
+DPK_HD void td_sort_serial(double *v, int n) {
+    for (int i = 1; i < n; i++) {
+        const double x = v[i];
+        int j = i;
+        while (j > 0 && x < v[j - 1]) { v[j] = v[j - 1]; j--; }
+        v[j] = x;
+    }
+}
+// Merged order of a fold: incoming entries (sorted) before old centroids (sorted) among equal means.  Incoming entry x
+// lands at its index + the old means below x; old mean y at its index + the incoming means <= y.
+DPK_HD int td_count_below(const double *v, int n, double x) {      // entries < x
+    int lo = 0, hi = n;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (v[mid] < x) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+DPK_HD int td_count_upto(const double *v, int n, double x) {       // entries <= x
+    int lo = 0, hi = n;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (!(x < v[mid])) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+// Entries one buffer takes before the add path folds: len(buf) + len(centroids) reaches TD_CAP first (at least one, as
+// MergingDigest.add appends after a compress that may leave TD_CAP centroids)
+DPK_HD int td_buffer_len(int C, int64_t left) {
+    const int64_t b = C < TD_CAP ? TD_CAP - C : 1;
+    return (int)(left < b ? left : b);
+}
+DPK_HD double td_between(double x1, double w1, double x2, double w2) {
+    const double lo = td_min(x1, x2), hi = td_max(x1, x2);
+    return td_max(lo, td_min(hi, td_div(td_add(td_mul(x1, w1), td_mul(x2, w2)), td_add(w1, w2))));
+}
+// MergingDigest.quantile(q) of a compressed digest: c centroids, merged weight mw, lo / hi the extreme means seen
+DPK_HD double td_quantile(const double *ms, const double *ws, int c, double mw, double lo, double hi, double q) {
+    if (c == 0) return NAN;
+    if (c == 1) return ms[0];
+    const double target = td_mul(q, mw);
+    if (target < td_div(ws[0], 2.0)) return td_add(lo, td_mul(td_div(td_mul(2.0, target), ws[0]), td_sub(ms[0], lo)));
+    double seen = td_div(ws[0], 2.0);
+    for (int i = 0; i < c - 1; i++) {
+        const double end = td_add(seen, td_div(td_add(ws[i], ws[i + 1]), 2.0));
+        if (end > target) return td_between(ms[i], td_sub(end, target), ms[i + 1], td_sub(target, seen));
+        seen = end;
+    }
+    const double left = td_sub(td_sub(target, mw), td_div(ws[c - 1], 2.0));
+    return td_between(ms[c - 1], left, hi, td_sub(td_div(ws[c - 1], 2.0), left));
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

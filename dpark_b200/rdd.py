@@ -432,13 +432,24 @@ class RDD(object):
         """dpark/rdd.py:815-850: per key the requested percentiles of its values (t-digest).  The reference builds
         one digest per key and map task and merges them on the reduce side in fetch order; here the values of a key
         arrive grouped and ordered by (input partition, position), each carries its partition index, and the same
-        digests are built and merged in partition order -- one of the orders the reference may take."""
+        digests are built and merged in partition order -- one of the orders the reference may take.
+
+        A numeric ColumnarRDD in a one-process job, with sampleRate >= 1 and no func, is digested on the device
+        (dpark_b200/percentiles.py), with the same partitions, keys and percentiles, bit for bit, as this composition."""
         if sampleRate <= 0:
             raise ValueError("Sample Rate should be positive.")
+        from . import join, percentiles
+        if sampleRate >= 1.0 and func is None and join.device_path_applies([self]):
+            part = self._combine_partitioner(numSplits, fixSkew)
+            if isinstance(part, HashPartitioner):       # other partitioners: the group-by below refuses them
+                return percentiles.ColumnarPercentilesByKeyRDD(self, part, p)
         rdd = self if sampleRate >= 1.0 else self.sample(sampleRate)
         if func:
             rdd = rdd.mapValue(func)
+        return rdd._percentiles_rows(p, numSplits, taskMemory, fixSkew)
 
+    def _percentiles_rows(self, p, numSplits=None, taskMemory=None, fixSkew=-1):
+        """percentilesByKey's composition over the rows of self (already sampled and mapped)."""
         def quantiles_of(tagged):
             merged, current, digest = None, None, None
             for part, x in tagged:
@@ -453,7 +464,7 @@ class RDD(object):
                 merged.compress()
             return [merged.quantile(pp / 100.) for pp in p]
 
-        tagged = rdd.mapPartitionWithIndex(lambda i, it: ((k, (i, v)) for k, v in it))
+        tagged = self.mapPartitionWithIndex(lambda i, it: ((k, (i, v)) for k, v in it))
         return tagged.groupByKey(numSplits, taskMemory, fixSkew=fixSkew).mapValue(quantiles_of)
 
     def fold(self, zero, f):

@@ -405,6 +405,30 @@ int dpk_sort_cuts(const int64_t *sorted_w0, const int64_t *ids, const void *vals
 int dpk_sort_gather(const void *keys, int32_t key_bytes, const void *vals, int32_t val_bytes, const int64_t *ids,
                     int64_t n, void *out_keys, void *out_vals, dpk_stream_t stream);
 
+/* ---- f7: percentilesByKey (dpark/rdd.py:815-850) of a numeric value column ---------------------------------------------
+ * Per key and map split the t-digest MergingDigest().update(values) + compress() (dpark_b200/quantiles.py, compression
+ * 100), absorbed into the key's first one in split order, then quantile(q) -- bit for bit.  The group-by's CSR gives
+ * every key's row ids ids[n] in (split, position) order; the splits are blocks of `per` rows, so row id r lies in split
+ * r / per.  A segment is one (key, split) run of ids.
+ *   dpk_tdigest_heads : head[n] (uint8, zeroed by the caller) gets 1 at every segment's first row.
+ *   dpk_tdigest_build : seg_starts[nseg + 1] = the heads' positions, then n; seg_off[nseg + 1] = the exclusive scan of
+ *                       min(segment length, 209).  Segment s's digest: cent_n[s] centroids at cent_m / cent_w[seg_off[s]
+ *                       ..] (means, weights), lohi[2 s .. 2 s + 1] = the smallest / largest first / last mean its folds
+ *                       met.  val_kind DPK_K_I32 / I64 / F32 / F64, converted as Python's float().  work: nseg + 2
+ *                       int64 of scratch.
+ *   dpk_tdigest_merge : out[g * nq + j] = quantile(qs[j]) of key g's merged digest (group_starts[ngroups + 1]).
+ * Both set *flag (device int32, zeroed by the caller) to nonzero when a value is NaN, a centroid mean comes out NaN or
+ * below its predecessor, or a fold would stage more than 418 entries: the results are then void. */
+int dpk_tdigest_heads(const int64_t *ids, int64_t n, const int64_t *group_starts, int64_t ngroups, int64_t per,
+                      uint8_t *head, dpk_stream_t stream);
+int dpk_tdigest_build(const int64_t *ids, const void *vals, int32_t val_kind, const int64_t *seg_starts,
+                      const int64_t *seg_off, int64_t nseg, double *cent_m, double *cent_w, int32_t *cent_n,
+                      double *lohi, int64_t *work, int32_t *flag, dpk_stream_t stream);
+int dpk_tdigest_merge(const int64_t *group_starts, int64_t ngroups, const int64_t *seg_starts, const int64_t *seg_off,
+                      int64_t nseg, const int32_t *cent_n, const double *lohi, const double *cent_m,
+                      const double *cent_w, const double *qs, int32_t nq, double *out, int32_t *flag,
+                      dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
