@@ -38,7 +38,7 @@ EXPORTS = [
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
     "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
-    "dpk_tdigest_heads", "dpk_tdigest_build", "dpk_tdigest_merge",
+    "dpk_tdigest_heads", "dpk_tdigest_build", "dpk_tdigest_merge", "dpk_sample_bernoulli",
 ]
 
 _lib = None
@@ -116,6 +116,7 @@ def lib():
         L.dpk_tdigest_heads.argtypes = [vp, i64, vp, i64, i64, vp, vp]
         L.dpk_tdigest_build.argtypes = [vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp]
         L.dpk_tdigest_merge.argtypes = [vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i32, vp, vp, vp]
+        L.dpk_sample_bernoulli.argtypes = [vp, vp, i64, C.c_double, vp, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -816,6 +817,37 @@ def tdigest_merge(group_starts, seg_starts, seg_off, digests, qs, flag):
                                    _ptr(cnt), _ptr(lohi), _ptr(cm), _ptr(cw), _ptr(qs), nq, _ptr(out), _ptr(flag),
                                    _stream()))
     return out
+
+
+# ---- f8: Bernoulli sample ------------------------------------------------------------------
+MT_N = 624            # MT19937's state words
+
+
+def sample_bernoulli(states, ranges, frac, nrows):
+    """SampleRDD's keep rule on the device (dpk_sample_bernoulli): states int32 [S, 624] (the words' bits), ranges
+    int64 [S, 2] (row begin, end) -> (ids, counts): int64 device [nrows] holding split i's kept row ids in row order
+    from ranges[i, 0] on, and int64 device [S] their numbers."""
+    _need_cuda(states, ranges)
+    S = int(ranges.shape[0])
+    if states.dtype != torch.int32:
+        raise TypeError("MT19937 states must be int32 tensors holding the words' bits")
+    if tuple(states.shape) != (S, MT_N) or tuple(ranges.shape) != (S, 2) or ranges.dtype != torch.int64:
+        raise ValueError("states [S, 624] and ranges [S, 2] int64 expected")
+    ids = torch.empty(max(1, nrows), dtype=torch.int64, device=ranges.device)
+    counts = torch.zeros(S, dtype=torch.int64, device=ranges.device)
+    _check(lib().dpk_sample_bernoulli(_ptr(states), _ptr(ranges), S, float(frac), _ptr(ids), _ptr(counts), _stream()))
+    return ids, counts
+
+
+def gather_columns(keys, vals, ids):
+    """keys[ids], vals[ids] in their own dtypes, bits preserved, len(ids) rows (dpk_sort_gather)."""
+    _need_cuda(keys, vals, ids)
+    n = int(ids.numel())
+    ok = torch.empty(n, dtype=keys.dtype, device=keys.device)
+    ov = torch.empty(n, dtype=vals.dtype, device=vals.device)
+    _check(lib().dpk_sort_gather(_ptr(keys), keys.element_size(), _ptr(vals), vals.element_size(), _ptr(ids), n,
+                                 _ptr(ok), _ptr(ov), _stream()))
+    return ok, ov
 
 
 def set_option(name, value):

@@ -648,6 +648,38 @@ DPK_HD double td_quantile(const double *ms, const double *ws, int c, double mw, 
     return td_between(ms[c - 1], left, hi, td_sub(td_div(ws[c - 1], 2.0), left));
 }
 
+// ------------------------------------------------------------- f8: Bernoulli sample (dpk_sample.cu; tests/samplecheck.cu
+// runs the same functions on the CPU).  SampleRDD keeps row j of split i when the j-th random.Random(seed + i).random()
+// is <= frac.  That generator is CPython's MT19937 (Modules/_randommodule.c): exact integer arithmetic, replayed here
+// word for word from the 624-word state random.Random(seed + i).getstate() holds right after seeding (pos = 624, so the
+// first draw twists).  A twist rewrites mt[0..624) in index order; it runs in three phases whose elements depend only on
+// words of earlier phases or not yet rewritten ones:
+//   [0, 227)   : mt[i + 1] and mt[i + 397], all old;
+//   [227, 454) : mt[i + 1] old, mt[i - 227] from phase 1;
+//   [454, 624) : mt[i + 1] old except the new mt[0] for i = 623, mt[i - 227] from phase 2.
+// Within a phase element i reads the old mt[i + 1] that element i + 1 rewrites, so every read precedes every write.
+constexpr int MT_N = 624, MT_M = 397;
+constexpr int MT_DRAWS = MT_N / 2;     // random() takes two words; a twist yields 312 draws and no pair straddles two
+DPK_HD int mt_phase(int p) { return p < 3 ? p * (MT_N - MT_M) : MT_N; }   // phase p covers [mt_phase(p), mt_phase(p + 1))
+DPK_HD uint32_t mt_twist_elem(const uint32_t *mt, int i) {
+    const uint32_t y = (mt[i] & 0x80000000u) | (mt[i + 1 == MT_N ? 0 : i + 1] & 0x7fffffffu);
+    const int far = i + MT_M < MT_N ? i + MT_M : i + MT_M - MT_N;
+    return mt[far] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
+}
+DPK_HD uint32_t mt_temper(uint32_t y) {
+    y ^= y >> 11;
+    y ^= (y << 7) & 0x9d2c5680u;
+    y ^= (y << 15) & 0xefc60000u;
+    return y ^ (y >> 18);
+}
+// random_random: (a * 2^26 + b) / 2^53 with a = w0 >> 5, b = w1 >> 6.  Every step is exact (a * 2^26 + b < 2^53), so a
+// contracted FMA gives the same double.
+DPK_HD double mt_double(uint32_t w0, uint32_t w1) {
+    return ((double)(w0 >> 5) * 67108864.0 + (double)(w1 >> 6)) * (1.0 / 9007199254740992.0);
+}
+// rd.random() <= frac as Python compares two floats: a NaN frac keeps nothing
+DPK_HD bool sample_keep(double u, double frac) { return u <= frac; }
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

@@ -144,13 +144,15 @@ def percentiles_of_partitions(partitions, percents, compression=100):
     return [merged.quantile(p / 100.) for p in percents]
 
 
-def skew_thresholds(hash_partitions, splits):
-    """The thresholds `combineByKey(fixSkew=...)` derives (dpark/rdd.py:516-537): percentiles of the
-    key hashes at i*100/splits, NaNs dropped, ceil()-ed, strictly increasing.  Returns
-    (thresholds or None, effective number of splits)."""
+def skew_marks(splits):
+    """The percentiles `combineByKey(fixSkew=...)` queries (dpark/rdd.py:516-537): i*100/splits for 0 < i < splits."""
     step = 100. / splits
-    marks = [step * i for i in range(1, splits)]
-    pcts = percentiles_of_partitions(hash_partitions, marks)
+    return [step * i for i in range(1, splits)]
+
+
+def thresholds_of(pcts, splits):
+    """The thresholds from the percentiles at skew_marks(splits): NaNs dropped, ceil()-ed, strictly increasing.
+    Returns (thresholds or None, effective number of splits)."""
     if not pcts:
         return None, splits
     thr = []
@@ -161,3 +163,10 @@ def skew_thresholds(hash_partitions, splits):
         if not thr or p > thr[-1]:
             thr.append(p)
     return thr, len(thr) + 1
+
+
+def skew_thresholds(hash_partitions, splits):
+    """The thresholds `combineByKey(fixSkew=...)` derives (dpark/rdd.py:516-537): percentiles of the
+    key hashes at i*100/splits, NaNs dropped, ceil()-ed, strictly increasing.  Returns
+    (thresholds or None, effective number of splits)."""
+    return thresholds_of(percentiles_of_partitions(hash_partitions, skew_marks(splits)), splits)

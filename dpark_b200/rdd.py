@@ -205,7 +205,13 @@ class RDD(object):
 
     # ------------------------------------------------------------- the shuffle
     def sample(self, faction, withReplacement=False, seed=12345):
-        """dpark/rdd.py:267-268."""
+        """dpark/rdd.py:267-268.
+
+        A numeric ColumnarRDD in a one-process job, sampled without replacement by an int or float fraction, is sampled
+        on the device (dpark_b200/sampling.py), with the same splits and rows as SampleRDD."""
+        from . import sampling
+        if sampling.sample_applies(self, faction, withReplacement):
+            return sampling.ColumnarSampleRDD(self, faction, withReplacement, seed)
         return SampleRDD(self, faction, withReplacement, seed)
 
     def percentiles(self, p, sampleRate=1.0, func=None):
@@ -219,7 +225,20 @@ class RDD(object):
 
     def _skew_thresholds(self, splits, sampleRate):
         """Thresholds of combineByKey(fixSkew=sampleRate) (dpark/rdd.py:516-537): approximate percentiles of
-        portable_hash(key) over a sample of the rows.  The sampled keys of every partition are hashed on the
+        portable_hash(key) over a sample of the rows.
+
+        A numeric ColumnarRDD, or a union of them, in a one-process job is sampled, hashed and digested on the device
+        (dpark_b200/sampling.py), with the same thresholds as this composition."""
+        from . import sampling
+        inputs = sampling.thresholds_inputs(self, sampleRate)
+        if inputs is not None:
+            res = sampling.skew_thresholds(inputs, splits, sampleRate)
+            if res is not None:
+                return res
+        return self._skew_thresholds_rows(splits, sampleRate)
+
+    def _skew_thresholds_rows(self, splits, sampleRate):
+        """_skew_thresholds' composition over the rows: the sampled keys of every partition are hashed on the
         device in one launch; the digest arithmetic is the reference's (dpark_b200/quantiles.py)."""
         rdd = self if sampleRate >= 1.0 else self.sample(sampleRate)
         hashed = [columnar.hashes_of_keys([row[0] for row in part])

@@ -429,6 +429,14 @@ int dpk_tdigest_merge(const int64_t *group_starts, int64_t ngroups, const int64_
                       const double *cent_w, const double *qs, int32_t nq, double *out, int32_t *flag,
                       dpk_stream_t stream);
 
+/* ---- f8: Bernoulli sample (dpark/rdd.py:1379-1397 SampleRDD without replacement) ---------------------------------------
+ * Split i covers rows [ranges[2 i], ranges[2 i + 1]) and owns the MT19937 state states[624 i .. 624 i + 624), the first
+ * 624 words of random.Random(seed + i).getstate()[1] right after seeding (its position is 624).  Row j of the split is
+ * kept when the j-th random() of that generator is <= frac (a plain double compare: a NaN frac keeps nothing).
+ * out_ids[ranges[2 i] ..] gets split i's kept row ids in row order, out_counts[i] how many there are (device int64). */
+int dpk_sample_bernoulli(const uint32_t *states, const int64_t *ranges, int64_t nsplits, double frac,
+                         int64_t *out_ids, int64_t *out_counts, dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
