@@ -39,6 +39,7 @@ EXPORTS = [
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
     "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
     "dpk_tdigest_heads", "dpk_tdigest_build", "dpk_tdigest_merge", "dpk_sample_bernoulli",
+    "dpk_select_round", "dpk_select_compact", "dpk_select_tiles", "dpk_select_take", "dpk_uniq_insert", "dpk_uniq_emit",
 ]
 
 _lib = None
@@ -117,6 +118,13 @@ def lib():
         L.dpk_tdigest_build.argtypes = [vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp]
         L.dpk_tdigest_merge.argtypes = [vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, i32, vp, vp, vp]
         L.dpk_sample_bernoulli.argtypes = [vp, vp, i64, C.c_double, vp, vp, vp]
+        L.dpk_select_round.argtypes = [vp, vp, vp, i64, vp, vp, vp]
+        L.dpk_select_compact.argtypes = [vp, vp, vp, i64, vp, vp, vp]
+        L.dpk_select_tiles.restype = i64
+        L.dpk_select_tiles.argtypes = [i64]
+        L.dpk_select_take.argtypes = [vp, vp, i64, i64, vp, vp, vp, vp, vp]
+        L.dpk_uniq_insert.argtypes = [vp, i32, vp, i32, i64, vp, i64, vp, vp]
+        L.dpk_uniq_emit.argtypes = [vp, i64, vp, vp, vp, vp]
         L.dpk_prof_enable.argtypes = [ci]
         L.dpk_prof_get.argtypes = [ci, C.c_char_p, C.POINTER(C.c_float)]
         if L.dpk_abi_version() != 1:
@@ -848,6 +856,69 @@ def gather_columns(keys, vals, ids):
     _check(lib().dpk_sort_gather(_ptr(keys), keys.element_size(), _ptr(vals), vals.element_size(), _ptr(ids), n,
                                  _ptr(ok), _ptr(ov), _stream()))
     return ok, ov
+
+
+# ---- f9: top / hot select and the uniq table ------------------------------------------------------------------------
+SEL_SHIFT0 = 56       # 64 - SEL_BITS: the first digit of a word
+SEL_BUCKETS = 256
+
+
+def select_state(n, m):
+    """The select's device state and histogram before the first round (dpk_select_round): rank n among m rows."""
+    st = torch.zeros(16, dtype=torch.int64)
+    st[1], st[2], st[4] = SEL_SHIFT0, n, m
+    hist = torch.zeros(3 * SEL_BUCKETS, dtype=torch.int64)
+    hist[2 * SEL_BUCKETS:] = -1
+    return st, hist
+
+
+def select_round(w0, w1, cands, m, state, hist):
+    """One MSD radix round of the select over m candidates (cands None: rows 0 .. m-1); updates state (dpk_select_round)."""
+    _need_cuda(w0, w1, cands, state, hist)
+    _check(lib().dpk_select_round(_ptr(w0), _ptr(w1), _ptr(cands), m, _ptr(state), _ptr(hist), _stream()))
+
+
+def select_compact(w0, w1, cands, m, state, count):
+    """The `count` candidates of the bucket the last round chose, int64 device (dpk_select_compact)."""
+    _need_cuda(w0, w1, cands, state)
+    out = torch.empty(count, dtype=torch.int64, device=w0.device)
+    _check(lib().dpk_select_compact(_ptr(w0), _ptr(w1), _ptr(cands), m, _ptr(state), _ptr(out), _stream()))
+    return out
+
+
+def select_take(w0, w1, take, state):
+    """The `take` smallest rows by (w0[, w1], id) once the rounds are done, in row id order (dpk_select_take)."""
+    _need_cuda(w0, w1, state)
+    n, dev = int(w0.numel()), w0.device
+    tiles = int(lib().dpk_select_tiles(n))
+    lt = torch.empty(tiles, dtype=torch.int64, device=dev)
+    eq = torch.empty(tiles, dtype=torch.int64, device=dev)
+    out = torch.empty(take, dtype=torch.int64, device=dev)
+    _check(lib().dpk_select_take(_ptr(w0), _ptr(w1), n, take, _ptr(state), _ptr(lt), _ptr(eq), _ptr(out), _stream()))
+    return out
+
+
+def uniq_insert(keys, vals):
+    """The distinct-count table of the rows' (k, v) pairs (dpk_uniq_insert): (table, state) -- bcast_slots(n) int64
+    slots and int64 [2] whose [0] is 1 when a NaN occurred."""
+    _need_cuda(keys, vals)
+    n, dev = int(keys.numel()), keys.device
+    S = bcast_slots(n)
+    table = torch.full((S,), 0x7FFFFFFF, dtype=torch.int64, device=dev)
+    state = torch.zeros(2, dtype=torch.int64, device=dev)
+    _check(lib().dpk_uniq_insert(_ptr(keys), _KEY_KIND.get(keys.dtype, -1), _ptr(vals), _KEY_KIND.get(vals.dtype, -1), n,
+                                 _ptr(table), S, _ptr(state), _stream()))
+    return table, state
+
+
+def uniq_emit(table, state, n):
+    """(first, count): int64 device [n] whose first state[1] entries are every distinct pair's first row id and row
+    count, in slot order (dpk_uniq_emit)."""
+    _need_cuda(table, state)
+    first = torch.empty(max(1, n), dtype=torch.int64, device=table.device)
+    count = torch.empty(max(1, n), dtype=torch.int64, device=table.device)
+    _check(lib().dpk_uniq_emit(_ptr(table), int(table.numel()), _ptr(first), _ptr(count), _ptr(state), _stream()))
+    return first, count
 
 
 def set_option(name, value):

@@ -680,6 +680,139 @@ DPK_HD double mt_double(uint32_t w0, uint32_t w1) {
 // rd.random() <= frac as Python compares two floats: a NaN frac keeps nothing
 DPK_HD bool sample_keep(double u, double frac) { return u <= frac; }
 
+// ------------------------------------------------------------- f9: top / hot select and the uniq table (dpk_select.cu;
+// tests/selectcheck.cu runs the same functions on the CPU)
+// The n smallest rows by (w0[, w1], row id) of unsigned 64-bit order words (sort_word), found by an MSD radix select:
+// each round takes one 8-bit digit of the current word over the candidates, picks the bucket holding the need-th
+// smallest, and keeps that bucket's rows as the next candidates.  Per bucket the round also ORs and ANDs the words, so
+// the bits in which the bucket's rows differ are known: the next digit starts at the highest of them, and when none is
+// left the word of the threshold row is exact.  A round therefore fixes at least 8 more bits or finishes a word: at most
+// 8 rounds per word.
+constexpr int SEL_BITS = 8, SEL_BUCKETS = 1 << SEL_BITS;
+DPK_HD uint32_t sel_digit(uint64_t w, int32_t shift) { return (uint32_t)(w >> shift) & (SEL_BUCKETS - 1); }
+// the bucket that holds the need-th smallest (1 <= need <= sum of hist): the first b with hist[0..b] >= need;
+// *below = hist[0..b), the candidates in lower buckets
+DPK_HD int32_t sel_bucket(const int64_t *hist, int64_t need, int64_t *below) {
+    int64_t cum = 0;
+    int32_t b = 0;
+    for (; b < SEL_BUCKETS - 1 && cum + hist[b] < need; b++) cum += hist[b];
+    *below = cum;
+    return b;
+}
+// the next round's shift given the bits below the current digit in which the chosen bucket's rows differ (nonzero):
+// the digit whose top bit is the highest of them, clamped at bit 0
+DPK_HD int32_t sel_next_shift(uint64_t diff) {
+    int32_t hb = 63;
+    while (!((diff >> hb) & 1)) hb--;
+    return hb >= SEL_BITS - 1 ? hb - (SEL_BITS - 1) : 0;
+}
+// (w0, w1) against the threshold (t0, t1) with nw words: < 0 below, 0 equal, > 0 above (sort_cmp)
+DPK_HD int sel_cmp(uint64_t w0, uint64_t w1, uint64_t t0, uint64_t t1, int32_t nw) { return sort_cmp(w0, w1, t0, t1, nw); }
+// The select state (int64 [SEL_STATE]): the current word and digit shift, the rank sought among the candidates, the
+// rows already below the threshold, the chosen bucket's size, the threshold words, done, and the rule the chosen
+// bucket's rows match (word, mask, value: (w & mask) == value); ST_OUT is the compaction's counter.
+enum { ST_WORD, ST_SHIFT, ST_NEED, ST_BELOW, ST_COUNT, ST_T0, ST_T1, ST_DONE, ST_MWORD, ST_MMASK, ST_MVAL, ST_OUT,
+       SEL_STATE = 16 };
+// One round's decision from its histogram hist[3 * SEL_BUCKETS] (counts, ORs, ANDs of the candidates' words per
+// bucket); clears the histogram for the next round (ANDs to all ones).
+DPK_HD void sel_pick(int64_t *st, uint64_t *hist, int32_t nw) {
+    int64_t below;
+    const int32_t b = sel_bucket(reinterpret_cast<const int64_t *>(hist), st[ST_NEED], &below);
+    const int32_t wi = (int32_t)st[ST_WORD], shift = (int32_t)st[ST_SHIFT];
+    // the candidates agree on the bits above the digit (earlier rounds), so the bucket's rows agree on every bit >= shift
+    const uint64_t hi = ~0ull << shift;
+    const uint64_t orb = hist[SEL_BUCKETS + b], andb = hist[2 * SEL_BUCKETS + b];
+    const uint64_t diff = (orb ^ andb) & ~hi;
+    st[ST_BELOW] += below;
+    st[ST_NEED] -= below;
+    st[ST_COUNT] = (int64_t)hist[b];
+    st[ST_MWORD] = wi;
+    st[ST_T0 + wi] = (int64_t)andb;                      // exact once diff is 0; its bits >= shift are final already
+    if (diff == 0) {                                     // the bucket's rows agree on the whole word
+        st[ST_MMASK] = (int64_t)~0ull;
+        if (wi + 1 < nw) {
+            st[ST_WORD] = wi + 1;
+            st[ST_SHIFT] = 64 - SEL_BITS;
+        } else {
+            st[ST_DONE] = 1;
+        }
+    } else {
+        st[ST_MMASK] = (int64_t)hi;
+        st[ST_SHIFT] = sel_next_shift(diff);
+    }
+    st[ST_MVAL] = (int64_t)(andb & (uint64_t)st[ST_MMASK]);
+    st[ST_OUT] = 0;
+    for (int j = 0; j < SEL_BUCKETS; j++) {
+        hist[j] = 0;
+        hist[SEL_BUCKETS + j] = 0;
+        hist[2 * SEL_BUCKETS + j] = ~0ull;
+    }
+}
+
+// uniq: a row's (k, v) pair as the distinct table compares it.  Each element widened as Python sees it (sort_wide_bits:
+// ints to int64, floats to float64) and, for floats, -0.0 spelled 0.0 (Python's dict finds (0.0, v) under (-0.0, v)).
+// False for a NaN in either element, which no dict lookup finds (the caller raises).  An int column and a float column
+// never share a table, so int bits and float bits never meet.
+DPK_HD uint64_t uniq_canon(uint64_t wide_bits, bool is_float) {
+    return is_float && wide_bits == (1ull << 63) ? 0ull : wide_bits;
+}
+DPK_HD bool uniq_pair_bits(const void *keys, int32_t kkind, const void *vals, int32_t vkind, int64_t i, uint64_t *kb,
+                           uint64_t *vb) {
+    const bool fk = sort_kind_float(kkind), fv = sort_kind_float(vkind);
+    const uint64_t a = sort_wide_bits(keys, kkind, i), b = sort_wide_bits(vals, vkind, i);
+    *kb = uniq_canon(a, fk);
+    *vb = uniq_canon(b, fv);
+    return !((fk && sort_is_nan(a)) || (fv && sort_is_nan(b)));
+}
+// The table: bcast_slots(n) slots of {owner, count}, linear probing.  owner is UNIQ_EMPTY or the id of a row holding
+// the slot's pair -- the pair lives in the input columns, never in the table, so a claim is one 32-bit CAS and nothing
+// is published after it.  Race-free: an owner goes only from UNIQ_EMPTY to a row id and then to smaller ids of rows
+// with the same pair, and claims are never undone, so every row of a pair stops at the same slot (the first one of its
+// probe sequence that is empty or holds the pair when reached) and the final owner is the pair's first row.
+constexpr int32_t UNIQ_EMPTY = 0x7FFFFFFF;     // above every row id (n < 2^31 - 1 rows)
+struct __align__(8) UniqSlot {
+    int32_t owner;
+    uint32_t count;
+};
+// a pair's first slot: both words mixed (mix64), the value word first so (a, b) and (b, a) part
+DPK_HD uint64_t uniq_slot(uint64_t kb, uint64_t vb, uint64_t mask) { return mix64(kb ^ mix64(vb + 0x9E3779B97F4A7C15ull)) & mask; }
+// Row i (pair kb, vb) into the table: claim the first empty slot of its probe sequence, or join the slot whose owner
+// row holds the same pair.  On the device the claim is a CAS and the join an atomicMin / atomicAdd.
+DPK_HD void uniq_insert_row(UniqSlot *table, uint64_t mask, const void *keys, int32_t kkind, const void *vals,
+                            int32_t vkind, int32_t i, uint64_t kb, uint64_t vb) {
+    for (uint64_t s = uniq_slot(kb, vb, mask);; s = (s + 1) & mask) {
+#ifdef __CUDA_ARCH__
+        int32_t o = *reinterpret_cast<volatile int32_t *>(&table[s].owner);
+        if (o == UNIQ_EMPTY) {
+            o = atomicCAS(&table[s].owner, UNIQ_EMPTY, i);
+            if (o == UNIQ_EMPTY) {
+                atomicAdd(&table[s].count, 1u);
+                return;
+            }
+        }
+#else
+        const int32_t o = table[s].owner;
+        if (o == UNIQ_EMPTY) {
+            table[s].owner = i;
+            table[s].count = 1;
+            return;
+        }
+#endif
+        uint64_t ok, ov;
+        uniq_pair_bits(keys, kkind, vals, vkind, o, &ok, &ov);
+        if (ok == kb && ov == vb) {
+#ifdef __CUDA_ARCH__
+            if (i < o) atomicMin(&table[s].owner, i);
+            atomicAdd(&table[s].count, 1u);
+#else
+            if (i < o) table[s].owner = i;
+            table[s].count++;
+#endif
+            return;
+        }
+    }
+}
+
 // ------------------------------------------------------------- f4: tokeniser arithmetic (dpk_strings.cu)
 // str.split() without arguments on ASCII text: whitespace = ' ', \t \n \v \f \r, \x1c..\x1f
 constexpr int TK_BYTES = 16;   // bytes per thread

@@ -337,13 +337,31 @@ class RDD(object):
     def uniq(self, numSplits=None, taskMemory=None, rddconf=None):
         """dpark/rdd.py:383-385: the distinct elements, partitioned by their hash.  The reference merges `None`
         values with `lambda x, y: None`; the GPU shuffle needs a recognised op, so the placeholder value is 0
-        merged with `or` -- the keys and their partitions are the same."""
+        merged with `or` -- the keys and their partitions are the same.
+
+        A numeric ColumnarRDD in a one-process job, partitioned by a HashPartitioner, is deduplicated on the device
+        (dpark_b200/selecting.py): the same partitions and elements, each partition's elements in order of first
+        occurrence with the bits of that occurrence."""
+        from . import selecting
+        if selecting.uniq_applies(self):
+            part = selecting.device_partitioner(self, numSplits)
+            if part is not None:
+                return selecting.ColumnarUniqRDD(self, part)
         import operator
         return self.map(lambda x: (x, 0)).reduceByKey(operator.or_, numSplits, taskMemory, rddconf=rddconf) \
                    .map(lambda kv: kv[0])
 
     def top(self, n=10, key=None, reverse=False):
-        """dpark/rdd.py:387-394: the n largest (smallest with reverse) elements; per partition, then overall."""
+        """dpark/rdd.py:387-394: the n largest (smallest with reverse) elements; per partition, then overall.
+
+        A numeric ColumnarRDD in a one-process job, with an int n and the identity (key None), x[0] or x[1] as the key,
+        is selected on the device (dpark_b200/selecting.py): the same list, ties in (split, position) order.  A NaN in
+        an order column keeps this composition."""
+        from . import selecting
+        if selecting.top_applies(self, n, key):
+            res = selecting.top(self, n, key, reverse)
+            if res is not None:
+                return res
         import heapq
         pick = heapq.nsmallest if reverse else heapq.nlargest
         best = []
@@ -352,7 +370,15 @@ class RDD(object):
         return pick(n, best, key)
 
     def hot(self, n=10, numSplits=None, taskMemory=None, rddconf=None):
-        """dpark/rdd.py:396-398: the n most frequent elements with their counts."""
+        """dpark/rdd.py:396-398: the n most frequent elements with their counts.
+
+        A numeric ColumnarRDD in a one-process job, with an int n and a HashPartitioner, is counted on the device
+        (dpark_b200/selecting.py): a stable top n by count over uniq's order of the elements."""
+        from . import selecting
+        if selecting.hot_applies(self, n):
+            part = selecting.device_partitioner(self, numSplits)
+            if part is not None:
+                return selecting.hot(self, n, part)
         counts = self.map(lambda x: (x, 1)).reduceByKey(lambda a, b: a + b, numSplits, taskMemory, rddconf=rddconf)
         return counts.top(n, key=lambda kv: kv[1])
 

@@ -437,6 +437,38 @@ int dpk_tdigest_merge(const int64_t *group_starts, int64_t ngroups, const int64_
 int dpk_sample_bernoulli(const uint32_t *states, const int64_t *ranges, int64_t nsplits, double frac,
                          int64_t *out_ids, int64_t *out_counts, dpk_stream_t stream);
 
+/* ---- f9: top, uniq and hot (dpark/rdd.py:383-398) of a numeric (k, v) column pair --------------------------------------
+ * Stable select of the n smallest rows by (w0[, w1], row id), w0 / w1 unsigned 64-bit order words (int64 bits, e.g. from
+ * dpk_sort_keys; w1 NULL for one word).  state: int64 [16] on the device, set by the caller before the first round to
+ * zeros except state[1] = 56 (the first digit's shift), state[2] = n (the rank sought) and state[4] = the row count;
+ * hist: int64 [768], zeros in [0, 512) and all ones in [512, 768).
+ *   dpk_select_round   : one MSD radix round over the m candidates (cands[m] row ids; NULL: all rows 0 .. m-1): picks the
+ *                        8-bit bucket of the state[2]-th smallest.  Afterwards state[4] = the candidates in that bucket,
+ *                        state[7] = 1 when the threshold words state[5] / state[6] are exact, state[3] = the rows below
+ *                        them.  At most 8 rounds per word.
+ *   dpk_select_compact : out_cands[state[4]] = the candidates of the chosen bucket (any order), for the next round.
+ *   dpk_select_take    : once state[7] = 1, out_ids[take] = every row below the threshold and the first take - state[3]
+ *                        rows equal to it, in row id order (take = the n of the rounds, < n rows).  tile_lt / tile_eq:
+ *                        dpk_select_tiles(n) int64 of scratch each.
+ * Distinct (k, v) pairs with their counts: a pair is both elements widened (ints to int64, floats to float64) with -0.0
+ * spelled 0.0; column kinds DPK_K_I64 / I32 / F64 / F32, read in place.
+ *   dpk_uniq_insert : every row into table (nslots = bcast_slots(n) slots of 8 bytes; every int64 slot filled with
+ *                     0x7FFFFFFF by the caller).  state: int64 [2], zeroed by the caller; state[0] = 1 when a NaN occurs
+ *                     (those rows are left out).
+ *   dpk_uniq_emit   : out_first[d] / out_count[d] = the first row id and the row count of every distinct pair, in slot
+ *                     order; state[1] = the number of pairs.  out_first / out_count hold at least n entries. */
+int dpk_select_round(const int64_t *w0, const int64_t *w1, const int64_t *cands, int64_t m, int64_t *state,
+                     int64_t *hist, dpk_stream_t stream);
+int dpk_select_compact(const int64_t *w0, const int64_t *w1, const int64_t *cands, int64_t m, int64_t *state,
+                       int64_t *out_cands, dpk_stream_t stream);
+int64_t dpk_select_tiles(int64_t n);
+int dpk_select_take(const int64_t *w0, const int64_t *w1, int64_t n, int64_t take, const int64_t *state,
+                    int64_t *tile_lt, int64_t *tile_eq, int64_t *out_ids, dpk_stream_t stream);
+int dpk_uniq_insert(const void *keys, int32_t key_kind, const void *vals, int32_t val_kind, int64_t n, void *table,
+                    int64_t nslots, int64_t *state, dpk_stream_t stream);
+int dpk_uniq_emit(const void *table, int64_t nslots, int64_t *out_first, int64_t *out_count, int64_t *state,
+                  dpk_stream_t stream);
+
 /* ---- f4: device text ingest (dpark/rdd.py:1633-1711 TextFileRDD + the tokenising flatMap of examples/wc.py:10-12) ----
  * Tokens of an ASCII byte range that begins and ends on line boundaries = its maximal runs of non-whitespace bytes
  * (str.split() without arguments: ' ', \t \n \v \f \r, \x1c..\x1f).  dpk_tokenize_count writes the number of token
