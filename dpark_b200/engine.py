@@ -71,8 +71,8 @@ def run_shuffle(srdd):
                 return res
         splits = _gather_parent(srdd, True)
         return _run_reduce(splits, P, thr, srdd.op, dev)
-    from . import join
-    if join.device_path_applies([srdd.parent]):
+    from .rdd import device_path_applies
+    if device_path_applies([srdd.parent]):
         return _run_group_columns(srdd.parent, P, thr)
     splits = _gather_parent(srdd, False)
     return _run_group(splits, P, thr, dev)

@@ -26,20 +26,8 @@ match count), and after one scan of the counts dpk_bcast_emit writes the rows, l
 import torch
 
 from . import _native as nv
-from . import grouping, spmd
-from .rdd import RDD, ColumnarRDD, Split
-
-DTYPES = (torch.int32, torch.int64, torch.float32, torch.float64)
-
-
-def device_path_applies(rdds):
-    """True when a join, cogroup or groupByKey of rdds runs on the device: every input a ColumnarRDD (not a subclass),
-    one process, 1-D key and value columns of int32 / int64 / float32 / float64."""
-    if any(type(r) is not ColumnarRDD for r in rdds):
-        return False
-    if spmd.rank_world()[1] != 1:
-        return False
-    return all(t.dtype in DTYPES and t.dim() == 1 for r in rdds for t in (r.keys, r.vals))
+from . import grouping
+from .rdd import DeviceResultRDD, Split, device_path_applies
 
 
 def reject_nan_keys(key_columns):
@@ -90,37 +78,31 @@ def join_columns(left, right, P, thresholds, keep_left, keep_right):
     return [tuple(None if c is None else c[bounds[p]:bounds[p + 1]] for c in cols) for p in range(P)]
 
 
-class ColumnarJoinedRDD(RDD):
+class ColumnarJoinedRDD(DeviceResultRDD):
     """The result of join / leftOuterJoin / rightOuterJoin / outerJoin of two numeric ColumnarRDDs in a one-process
     job: the rows RDD._join's composition yields, computed on the GPU the first time a partition is asked for and
-    kept (like ShuffledRDD).  Like the flatMap it stands for, it has the cogroup's partitions and no partitioner."""
+    kept (like ShuffledRDD).  Like the flatMap it stands for, it has the cogroup's partitions and no partitioner.
+
+    columns(split) hands out CUDA tensors (keys, left, right, left_valid, right_valid).  Keys are int64 or float64,
+    values keep their input dtypes; a valid column is uint8 (0 = the side is missing, its value slot holds 0) and None
+    for a side the join kind never misses."""
 
     def __init__(self, left, right, part, keep_left, keep_right):
-        RDD.__init__(self, left.ctx)
+        DeviceResultRDD.__init__(self, left.ctx)
         self.left, self.right = left, right
         self.join_partitioner = part
         self.keep_left, self.keep_right = keep_left, keep_right
         self._splits = [Split(i) for i in range(part.numPartitions)]
-        self._result = None
 
     def parents(self):
         return [self.left, self.right]
 
-    def _materialize(self):
-        if self._result is None:
-            p = self.join_partitioner
-            self._result = join_columns(self.left, self.right, p.numPartitions, p.thresholds, self.keep_left,
-                                        self.keep_right)
-        return self._result
+    def _run(self):
+        p = self.join_partitioner
+        return join_columns(self.left, self.right, p.numPartitions, p.thresholds, self.keep_left, self.keep_right)
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, left, right, left_valid, right_valid).  Keys are int64
-        or float64, values keep their input dtypes; a valid column is uint8 (0 = the side is missing, its value slot
-        holds 0) and None for a side the join kind never misses."""
-        return self._materialize()[split.index]
-
-    def compute(self, split):
-        keys, left, right, lvalid, rvalid = self.columns(split)
+    def _rows(self, columns):
+        keys, left, right, lvalid, rvalid = columns
         ls, rs = left.cpu().tolist(), right.cpu().tolist()
         if lvalid is not None:
             ls = [x if ok else None for x, ok in zip(ls, lvalid.cpu().tolist())]
@@ -130,8 +112,8 @@ class ColumnarJoinedRDD(RDD):
 
 
 def inner_join_applies(big, small):
-    """True when big.innerJoin(small) runs on the device: device_path_applies, and not int keys on one side with float
-    keys on the other (both non-empty; Python's 1 == 1.0 is not the device's equality)."""
+    """True when big.innerJoin(small) runs on the device: rdd.device_path_applies, and not int keys on one side with
+    float keys on the other (both non-empty; Python's 1 == 1.0 is not the device's equality)."""
     if not device_path_applies([big, small]):
         return False
     sides = [r.keys for r in (big, small) if r.keys.numel()]
@@ -168,32 +150,27 @@ def inner_join_columns(big, small):
     return [tuple(c[rows[s]:rows[s + 1]] for c in cols) for s in range(len(big.splits))]
 
 
-class ColumnarInnerJoinedRDD(RDD):
+class ColumnarInnerJoinedRDD(DeviceResultRDD):
     """The result of big.innerJoin(small) of two numeric ColumnarRDDs in a one-process job: the rows RDD.innerJoin's
     flatMap yields, computed on the GPU the first time a partition is asked for and kept.  Like the flatMap it has
-    big's splits and no partitioner."""
+    big's splits and no partitioner.
+
+    columns(split) hands out the rows of big's split `split` as CUDA tensors (keys, left, right): keys in big's key
+    dtype with their own bits, left in big's value dtype, right in small's value dtype."""
 
     def __init__(self, big, small):
-        RDD.__init__(self, big.ctx)
+        DeviceResultRDD.__init__(self, big.ctx)
         self.big, self.small = big, small
         self._splits = [Split(i) for i in range(len(big.splits))]
-        self._result = None
 
     def parents(self):
         return [self.big, self.small]
 
-    def _materialize(self):
-        if self._result is None:
-            self._result = inner_join_columns(self.big, self.small)
-        return self._result
+    def _run(self):
+        return inner_join_columns(self.big, self.small)
 
-    def columns(self, split):
-        """Extension: partition `split` (the rows of big's split `split`) as CUDA tensors (keys, left, right): keys in
-        big's key dtype with their own bits, left in big's value dtype, right in small's value dtype."""
-        return self._materialize()[split.index]
-
-    def compute(self, split):
-        keys, left, right = self.columns(split)
+    def _rows(self, columns):
+        keys, left, right = columns
         return zip(keys.cpu().tolist(), zip(left.cpu().tolist(), right.cpu().tolist()))
 
 
@@ -242,34 +219,29 @@ def partition_slices(gk, off, cols, pg, rows):
              tuple(c[r[p]:r[p + 1]] for c, r in zip(cols, rows))) for p in range(len(pg) - 1)]
 
 
-class ColumnarCoGroupedRDD(RDD):
+class ColumnarCoGroupedRDD(DeviceResultRDD):
     """The result of groupWith / cogroup of numeric ColumnarRDDs in a one-process job: per key one value list per
     input, the rows CoGroupedRDD yields, computed on the GPU the first time a partition is asked for and kept.  It has
-    the cogroup's partitioner, so mapValue keeps it and a later groupWith reads it as a narrow dependency."""
+    the cogroup's partitioner, so mapValue keeps it and a later groupWith reads it as a narrow dependency.
+
+    columns(split) hands out CUDA tensors (keys, offsets, values): keys int64 or float64, offsets int64 [N, keys + 1],
+    values a tuple of N columns in the inputs' dtypes (see cogroup_columns)."""
 
     def __init__(self, rdds, part):
-        RDD.__init__(self, rdds[0].ctx)
+        DeviceResultRDD.__init__(self, rdds[0].ctx)
         self.rdds = list(rdds)
         self.partitioner = part
         self._splits = [Split(i) for i in range(part.numPartitions)]
-        self._result = None
 
     def parents(self):
         return list(self.rdds)
 
-    def _materialize(self):
-        if self._result is None:
-            p = self.partitioner
-            self._result = cogroup_columns(self.rdds, p.numPartitions, p.thresholds)
-        return self._result
+    def _run(self):
+        p = self.partitioner
+        return cogroup_columns(self.rdds, p.numPartitions, p.thresholds)
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, offsets, values): keys int64 or float64, offsets int64
-        [N, keys + 1], values a tuple of N columns in the inputs' dtypes (see cogroup_columns)."""
-        return self._materialize()[split.index]
-
-    def compute(self, split):
-        keys, offsets, values = self.columns(split)
+    def _rows(self, columns):
+        keys, offsets, values = columns
         off = offsets.cpu().tolist()
         vals = [v.cpu().tolist() for v in values]
         groups = zip(*[[vs[o[j]:o[j + 1]] for j in range(len(o) - 1)] for o, vs in zip(off, vals)])

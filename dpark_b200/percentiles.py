@@ -23,7 +23,7 @@ import torch
 
 from . import _native as nv
 from . import grouping, join
-from .rdd import RDD, Split
+from .rdd import DeviceResultRDD, Split
 
 TD_CAP = nv.TD_CAP
 
@@ -67,50 +67,34 @@ def percentiles_columns(rdd, P, thresholds, qs):
     return [(k, v) for k, _, (v,) in join.partition_slices(gk, gs.unsqueeze(0), [out], pg, rows)]
 
 
-class ColumnarPercentilesByKeyRDD(RDD):
+class ColumnarPercentilesByKeyRDD(DeviceResultRDD):
     """The result of percentilesByKey(p) of a numeric ColumnarRDD in a one-process job: per key the list of its
     percentiles, the rows of the composition (RDD._percentiles_rows), computed on the GPU the first time a partition is
     asked for and kept.  It has the group-by's partitioner, so mapValue keeps it and a later groupWith reads it as a
-    narrow dependency."""
+    narrow dependency.  columns(split) hands out CUDA tensors (keys, quantiles): keys int64 or float64, quantiles
+    float64 [keys, len(p)]; where the module docstring says so the composition's rows stand."""
 
     def __init__(self, parent, part, p):
-        RDD.__init__(self, parent.ctx)
+        DeviceResultRDD.__init__(self, parent.ctx)
         self.parent = parent
         self.partitioner = part
         self.p = list(p)
         self._splits = [Split(i) for i in range(part.numPartitions)]
-        self._result = None
 
     def parents(self):
         return [self.parent]
 
-    def _materialize(self):
-        """The partitions' columns, or the composition RDD whose rows stand."""
-        if self._result is None:
-            part = self.partitioner
-            qs = [pp / 100. for pp in self.p]
-            res = None
-            if all(0 <= q <= 1 for q in qs) or self.parent.keys.numel() == 0:
-                res = percentiles_columns(self.parent, part.numPartitions, part.thresholds, qs)
-            self._result = res if res is not None else self.parent._percentiles_rows(self.p, part)
-        return self._result
+    def _run(self):
+        part = self.partitioner
+        qs = [pp / 100. for pp in self.p]
+        if all(0 <= q <= 1 for q in qs) or self.parent.keys.numel() == 0:
+            return percentiles_columns(self.parent, part.numPartitions, part.thresholds, qs)
+        return None
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, quantiles): keys int64 or float64, quantiles float64
-        [keys, len(p)]."""
-        res = self._materialize()
-        if isinstance(res, RDD):
-            from .engine import _device
-            dev = _device()
-            rows = list(res.iterator(res.splits[split.index]))
-            kdt = torch.float64 if self.parent.keys.dtype.is_floating_point else torch.int64
-            return (torch.tensor([k for k, _ in rows], dtype=kdt, device=dev),
-                    torch.tensor([qs for _, qs in rows], dtype=torch.float64, device=dev).view(len(rows), len(self.p)))
-        return res[split.index]
+    def _composition(self):
+        return self.parent._percentiles_rows(self.p, self.partitioner)
 
-    def compute(self, split):
-        res = self._materialize()
-        if isinstance(res, RDD):
-            return res.iterator(res.splits[split.index])
-        keys, quant = res[split.index]
-        return zip(keys.cpu().tolist(), quant.cpu().tolist())
+    def _columns_of_rows(self, rows, dev):
+        kdt = torch.float64 if self.parent.keys.dtype.is_floating_point else torch.int64
+        return (torch.tensor([k for k, _ in rows], dtype=kdt, device=dev),
+                torch.tensor([qs for _, qs in rows], dtype=torch.float64, device=dev).view(len(rows), len(self.p)))

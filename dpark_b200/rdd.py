@@ -263,6 +263,12 @@ class RDD(object):
             splits = HashPartitioner(splits, thresholds=thresh)
         return splits
 
+    def _device_partitioner(self, numSplits, fixSkew=-1):
+        """_combine_partitioner(numSplits, fixSkew) if a device group-by can take it -- a HashPartitioner -- else None
+        (the composition's group-by refuses every other partitioner as well)."""
+        part = self._combine_partitioner(numSplits, fixSkew)
+        return part if isinstance(part, HashPartitioner) else None
+
     def reduceByKey(self, func, numSplits=None, taskMemory=None, fixSkew=-1, rddconf=None):
         """dpark/rdd.py:543-545."""
         aggregator = Aggregator(lambda x: x, func, func)
@@ -281,8 +287,8 @@ class RDD(object):
             others = [others]
         others = list(others)
         part = self._cogroup_partitioner(others, numSplits, fixSkew)
-        from . import join
-        if join.device_path_applies([self] + others):
+        if device_path_applies([self] + others):
+            from . import join
             return join.ColumnarCoGroupedRDD([self] + others, part)
         return CoGroupedRDD([self] + others, part, taskMemory, rddconf=rddconf)
 
@@ -319,8 +325,8 @@ class RDD(object):
         Two numeric ColumnarRDDs in a one-process job are joined on the device (dpark_b200/join.py), with the same
         partitions, rows and order as this composition."""
         keep_left, keep_right = 1 in keeps, 2 in keeps
-        from . import join
-        if join.device_path_applies([self, other]):
+        if device_path_applies([self, other]):
+            from . import join
             return join.ColumnarJoinedRDD(self, other, self._cogroup_partitioner([other], numSplits, fixSkew),
                                           keep_left, keep_right)
 
@@ -344,7 +350,7 @@ class RDD(object):
         occurrence with the bits of that occurrence."""
         from . import selecting
         if selecting.uniq_applies(self):
-            part = selecting.device_partitioner(self, numSplits)
+            part = self._device_partitioner(numSplits)
             if part is not None:
                 return selecting.ColumnarUniqRDD(self, part)
         import operator
@@ -376,7 +382,7 @@ class RDD(object):
         (dpark_b200/selecting.py): a stable top n by count over uniq's order of the elements."""
         from . import selecting
         if selecting.hot_applies(self, n):
-            part = selecting.device_partitioner(self, numSplits)
+            part = self._device_partitioner(numSplits)
             if part is not None:
                 return selecting.hot(self, n, part)
         counts = self.map(lambda x: (x, 1)).reduceByKey(lambda a, b: a + b, numSplits, taskMemory, rddconf=rddconf)
@@ -396,10 +402,10 @@ class RDD(object):
         the device (dpark_b200/topk.py), with the same partitions, keys, values and order as this composition."""
         if top_n <= 0:
             raise AssertionError("top_n must be positive")
-        from . import join, topk
-        if order_func is None and type(top_n) is int and top_n <= topk.TOPK_MAX_N and join.device_path_applies([self]):
-            part = self._combine_partitioner(num_splits, fixSkew)
-            if isinstance(part, HashPartitioner):       # other partitioners: the group-by below refuses them
+        from . import topk
+        if order_func is None and type(top_n) is int and top_n <= topk.TOPK_MAX_N and device_path_applies([self]):
+            part = self._device_partitioner(num_splits, fixSkew)
+            if part is not None:
                 return topk.ColumnarTopByKeyRDD(self, part, top_n, reverse)
         return self.groupByKey(num_splits, task_memory, fixSkew=fixSkew).mapValue(top_values(top_n, order_func, reverse))
 
@@ -483,10 +489,10 @@ class RDD(object):
         (dpark_b200/percentiles.py), with the same partitions, keys and percentiles, bit for bit, as this composition."""
         if sampleRate <= 0:
             raise ValueError("Sample Rate should be positive.")
-        from . import join, percentiles
-        if sampleRate >= 1.0 and func is None and join.device_path_applies([self]):
-            part = self._combine_partitioner(numSplits, fixSkew)
-            if isinstance(part, HashPartitioner):       # other partitioners: the group-by below refuses them
+        from . import percentiles
+        if sampleRate >= 1.0 and func is None and device_path_applies([self]):
+            part = self._device_partitioner(numSplits, fixSkew)
+            if part is not None:
                 return percentiles.ColumnarPercentilesByKeyRDD(self, part, p)
         rdd = self if sampleRate >= 1.0 else self.sample(sampleRate)
         if func:
@@ -708,6 +714,60 @@ class ColumnarRDD(RDD):
     def compute(self, split):
         k, v = self.columns(split)
         return zip(k.cpu().tolist(), v.cpu().tolist())
+
+
+def device_path_applies(rdds, max_rows=None):
+    """True when a columnar operator over rdds may run on the device: every input a ColumnarRDD (not a subclass), one
+    process, 1-D key and value columns of int32 / int64 / float32 / float64, and at most max_rows rows in each input
+    when a cap is given.  Each operator adds its own argument checks (sorting.device_sort_applies, ...)."""
+    import torch
+    from . import spmd
+    if any(type(r) is not ColumnarRDD for r in rdds) or spmd.rank_world()[1] != 1:
+        return False
+    if max_rows is not None and any(int(r.keys.numel()) > max_rows for r in rdds):
+        return False
+    dtypes = (torch.int32, torch.int64, torch.float32, torch.float64)
+    return all(t.dtype in dtypes and t.dim() == 1 for r in rdds for t in (r.keys, r.vals))
+
+
+class DeviceResultRDD(RDD):
+    """The result of a columnar operator on the device: every partition is computed in one go the first time any
+    partition is asked for, and kept (like ShuffledRDD).  A subclass gives
+
+      _run()                   the device result, or None when the composition's rows must stand instead;
+      _rows(columns)           one partition's columns as the composition's rows (by default (keys, values) pairs);
+      _part(result, index)     one partition's columns cut from the result (by default result[index]);
+      _composition()           and _columns_of_rows(rows, device), where _run may return None.
+
+    columns(split) hands out the partition as CUDA tensors, also when the composition stands."""
+
+    _result = None          # the device result, or the composition RDD whose rows stand
+
+    def _materialize(self):
+        if self._result is None:
+            res = self._run()
+            self._result = res if res is not None else self._composition()
+        return self._result
+
+    def _part(self, result, index):
+        return result[index]
+
+    def _rows(self, columns):
+        keys, vals = columns
+        return zip(keys.cpu().tolist(), vals.cpu().tolist())
+
+    def columns(self, split):
+        res = self._materialize()
+        if isinstance(res, RDD):
+            from .engine import _device
+            return self._columns_of_rows(list(res.iterator(res.splits[split.index])), _device())
+        return self._part(res, split.index)
+
+    def compute(self, split):
+        res = self._materialize()
+        if isinstance(res, RDD):
+            return res.iterator(res.splits[split.index])
+        return self._rows(self._part(res, split.index))
 
 
 class TextFileRDD(RDD):

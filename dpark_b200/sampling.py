@@ -29,8 +29,8 @@ import numpy as np
 import torch
 
 from . import _native as nv
-from . import join, quantiles
-from .rdd import ColumnarRDD, SampleRDD, UnionRDD
+from . import quantiles
+from .rdd import ColumnarRDD, DeviceResultRDD, SampleRDD, UnionRDD, device_path_applies
 
 SKEW_SEED = 12345         # RDD.sample's default seed, the one _skew_thresholds samples with
 NAN_KEYS = "NaN keys are not supported (CPython hashes NaN by identity)"
@@ -42,8 +42,8 @@ def _number(x):
 
 def sample_applies(rdd, frac, withReplacement):
     """True when rdd.sample(frac, withReplacement) runs on the device: a numeric ColumnarRDD in a one-process job
-    (join.device_path_applies), without replacement, with an int or float fraction."""
-    return not withReplacement and _number(frac) and join.device_path_applies([rdd])
+    (rdd.device_path_applies), without replacement, with an int or float fraction."""
+    return not withReplacement and _number(frac) and device_path_applies([rdd])
 
 
 def thresholds_inputs(rdd, rate):
@@ -56,7 +56,7 @@ def thresholds_inputs(rdd, rate):
         inputs = list(rdd.rdds)
     else:
         return None
-    return inputs if _number(rate) and join.device_path_applies(inputs) else None
+    return inputs if _number(rate) and device_path_applies(inputs) else None
 
 
 def mt_states(seed, n):
@@ -151,29 +151,17 @@ def skew_thresholds(inputs, splits, rate):
     return quantiles.thresholds_of(out.view(-1).cpu().tolist(), splits)
 
 
-class ColumnarSampleRDD(SampleRDD):
+class ColumnarSampleRDD(DeviceResultRDD, SampleRDD):
     """rdd.sample(frac, False, seed) of a numeric ColumnarRDD in a one-process job: the parent's splits, no partitioner,
     and SampleRDD's rows, drawn on the GPU the first time a partition is asked for and kept.  columns(split) hands out
     the kept rows as CUDA tensors in the parent's dtypes and bits."""
 
-    def __init__(self, prev, frac, withReplacement, seed):
-        SampleRDD.__init__(self, prev, frac, withReplacement, seed)
-        self._result = None
+    def _run(self):
+        p = self.prev
+        ids, counts = bernoulli([(s.begin, s.end) for s in p.splits], int(p.keys.numel()), self.frac, self.seed)
+        keys, vals = nv.gather_columns(p.keys.to(ids.device).contiguous(), p.vals.to(ids.device).contiguous(), ids)
+        return keys, vals, [0] + list(itertools.accumulate(counts))
 
-    def _materialize(self):
-        if self._result is None:
-            p = self.prev
-            ids, counts = bernoulli([(s.begin, s.end) for s in p.splits], int(p.keys.numel()), self.frac, self.seed)
-            keys, vals = nv.gather_columns(p.keys.to(ids.device).contiguous(), p.vals.to(ids.device).contiguous(), ids)
-            self._result = keys, vals, [0] + list(itertools.accumulate(counts))
-        return self._result
-
-    def columns(self, split):
-        """Extension: the kept rows of `split` as CUDA tensors (keys, vals)."""
-        keys, vals, off = self._materialize()
-        i = split.index
+    def _part(self, result, i):
+        keys, vals, off = result
         return keys[off[i]:off[i + 1]], vals[off[i]:off[i + 1]]
-
-    def compute(self, split):
-        k, v = self.columns(split)
-        return zip(k.cpu().tolist(), v.cpu().tolist())

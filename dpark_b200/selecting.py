@@ -13,9 +13,8 @@ A NaN in an order column keeps top's composition; a NaN in either column raises 
 import torch
 
 from . import _native as nv
-from . import join, shuffle, sorting
-from .dependency import HashPartitioner
-from .rdd import RDD, Split
+from . import shuffle, sorting
+from .rdd import RDD, DeviceResultRDD, Split, device_path_applies
 
 NAN_KEYS = "NaN keys are not supported (CPython hashes NaN by identity)"
 MAX_UNIQ_ROWS = (1 << 31) - 2       # row ids stay below the table's empty mark 0x7FFFFFFF
@@ -29,21 +28,23 @@ def top_order(key):
 
 
 def top_applies(rdd, n, key):
-    """True when rdd.top(n, key, reverse) runs on the device: a numeric ColumnarRDD in a one-process job
-    (join.device_path_applies), an int n, at most sorting.MAX_ROWS rows and a recognised key."""
-    return (type(n) is int and join.device_path_applies([rdd]) and int(rdd.keys.numel()) <= sorting.MAX_ROWS
-            and top_order(key) is not None)
+    """True when rdd.top(n, key, reverse) runs on the device: an int n, a numeric ColumnarRDD in a one-process job
+    (rdd.device_path_applies) with at most sorting.MAX_ROWS rows, and a recognised key."""
+    return type(n) is int and device_path_applies([rdd], sorting.MAX_ROWS) and top_order(key) is not None
 
 
 def uniq_applies(rdd):
     """True when rdd.uniq(...) runs on the device (given a HashPartitioner): a numeric ColumnarRDD in a one-process job
-    with at most MAX_UNIQ_ROWS rows."""
-    return join.device_path_applies([rdd]) and int(rdd.keys.numel()) <= MAX_UNIQ_ROWS
+    (rdd.device_path_applies) with at most MAX_UNIQ_ROWS rows."""
+    return device_path_applies([rdd], MAX_UNIQ_ROWS)
 
 
 def hot_applies(rdd, n):
     """True when rdd.hot(n, ...) runs on the device (given a HashPartitioner): uniq_applies and an int n."""
     return type(n) is int and uniq_applies(rdd)
+
+
+device_partitioner = RDD._device_partitioner     # (rdd, numSplits): the HashPartitioner uniq / hot take, or None
 
 
 def select_smallest(w0, w1, n):
@@ -138,38 +139,23 @@ def hot(rdd, n, part):
     return [((a, b), c) for a, b, c in zip(hk.cpu().tolist(), hv.cpu().tolist(), count[ids].cpu().tolist())]
 
 
-class ColumnarUniqRDD(RDD):
+class ColumnarUniqRDD(DeviceResultRDD):
     """rdd.uniq(numSplits) of a numeric ColumnarRDD in a one-process job: the composition's partition count and no
     partitioner; partition p holds the distinct (k, v) pairs with portable_hash((k, v)) % P == p, in order of first
-    occurrence, each with its first row's bits.  Computed on the GPU the first time a partition is asked for and kept."""
+    occurrence, each with its first row's bits.  Computed on the GPU the first time a partition is asked for and kept;
+    columns(split) hands out CUDA tensors (keys, values) in the input dtypes."""
 
     def __init__(self, parent, part):
-        RDD.__init__(self, parent.ctx)
+        DeviceResultRDD.__init__(self, parent.ctx)
         self.parent, self.part = parent, part
         self._splits = [Split(i) for i in range(part.numPartitions)]
-        self._result = None
 
     def parents(self):
         return [self.parent]
 
-    def _materialize(self):
-        if self._result is None:
-            self._result = distinct(self.parent, self.part)
-        return self._result
+    def _run(self):
+        return distinct(self.parent, self.part)
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, values) in the input dtypes."""
-        keys, vals, _, off = self._materialize()
-        i = split.index
+    def _part(self, result, i):
+        keys, vals, _, off = result
         return keys[off[i]:off[i + 1]], vals[off[i]:off[i + 1]]
-
-    def compute(self, split):
-        keys, vals = self.columns(split)
-        return zip(keys.cpu().tolist(), vals.cpu().tolist())
-
-
-def device_partitioner(rdd, numSplits):
-    """The composition's partitioner of uniq / hot (_combine_partitioner(numSplits, -1)) if the device path can take
-    it -- a HashPartitioner -- else None."""
-    part = rdd._combine_partitioner(numSplits, -1)
-    return part if isinstance(part, HashPartitioner) else None

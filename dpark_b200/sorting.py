@@ -15,8 +15,8 @@ import struct
 import torch
 
 from . import _native as nv
-from . import join, shuffle
-from .rdd import RDD, Split, range_bounds
+from . import shuffle
+from .rdd import DeviceResultRDD, Split, device_path_applies, range_bounds
 from .textingest import _same
 
 _t_identity = lambda x: x           # noqa: E731
@@ -46,9 +46,9 @@ def order_of(key):
 
 
 def device_sort_applies(rdd, key):
-    """True when rdd.sort(key, ...) runs on the device: join.device_path_applies (a plain ColumnarRDD in a one-process
-    job with 1-D int32 / int64 / float32 / float64 columns), fewer than 2^31 rows and a recognised key."""
-    return join.device_path_applies([rdd]) and int(rdd.keys.numel()) <= MAX_ROWS and order_of(key) is not None
+    """True when rdd.sort(key, ...) runs on the device: rdd.device_path_applies (a plain ColumnarRDD in a one-process
+    job with 1-D int32 / int64 / float32 / float64 columns) with fewer than 2^31 rows, and a recognised key."""
+    return device_path_applies([rdd], MAX_ROWS) and order_of(key) is not None
 
 
 def sample_bounds(rdd, key, reverse, numSplits):
@@ -107,48 +107,31 @@ def sort_columns(rdd, order, reverse, bounds):
     return [(sk[starts[p]:starts[p + 1]], sv[starts[p]:starts[p + 1]]) for p in range(P)]
 
 
-class ColumnarSortedRDD(RDD):
+class ColumnarSortedRDD(DeviceResultRDD):
     """The result of sort(key, reverse, numSplits) of a numeric ColumnarRDD in a one-process job with a recognised key:
     the partitions of RDD.sort's composition, computed on the GPU the first time a partition is asked for and kept.  The
     range bounds are sampled at construction, as the composition samples them.  Like the composition's mapPartitions
-    it has no partitioner."""
+    it has no partitioner.  columns(split) hands out CUDA tensors (keys, values) in the input dtypes; when an order
+    column holds a NaN the composition's rows stand."""
 
     def __init__(self, parent, key, reverse, numSplits, taskMemory=None, rddconf=None):
-        RDD.__init__(self, parent.ctx)
+        DeviceResultRDD.__init__(self, parent.ctx)
         self.parent = parent
         self.key, self.reverse, self.numSplits = key, reverse, numSplits
         self.taskMemory, self.sort_rddconf = taskMemory, rddconf
         self.order = order_of(key)
         self.bounds = sample_bounds(parent, key, reverse, numSplits)
         self._splits = [Split(i) for i in range(len(self.bounds) + 1)]
-        self._result = None
 
     def parents(self):
         return [self.parent]
 
-    def _materialize(self):
-        """The partitions' columns, or, when an order column holds a NaN, the composition RDD whose rows stand."""
-        if self._result is None:
-            res = sort_columns(self.parent, self.order, self.reverse, self.bounds)
-            if res is None:
-                res = self.parent._sort_rows(self.key, self.reverse, self.numSplits, self.taskMemory, self.sort_rddconf)
-            self._result = res
-        return self._result
+    def _run(self):
+        return sort_columns(self.parent, self.order, self.reverse, self.bounds)
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, values) in the input dtypes."""
-        res = self._materialize()
-        if isinstance(res, RDD):
-            from .engine import _device
-            dev = _device()
-            rows = list(res.iterator(res.splits[split.index]))
-            return (torch.tensor([k for k, _ in rows], dtype=self.parent.keys.dtype, device=dev),
-                    torch.tensor([v for _, v in rows], dtype=self.parent.vals.dtype, device=dev))
-        return res[split.index]
+    def _composition(self):
+        return self.parent._sort_rows(self.key, self.reverse, self.numSplits, self.taskMemory, self.sort_rddconf)
 
-    def compute(self, split):
-        res = self._materialize()
-        if isinstance(res, RDD):
-            return res.iterator(res.splits[split.index])
-        keys, vals = res[split.index]
-        return zip(keys.cpu().tolist(), vals.cpu().tolist())
+    def _columns_of_rows(self, rows, dev):
+        return (torch.tensor([k for k, _ in rows], dtype=self.parent.keys.dtype, device=dev),
+                torch.tensor([v for _, v in rows], dtype=self.parent.vals.dtype, device=dev))

@@ -21,7 +21,7 @@ import torch
 
 from . import _native as nv
 from . import grouping, join
-from .rdd import RDD, Split, top_values
+from .rdd import DeviceResultRDD, Split, top_values
 
 TOPK_MAX_N = nv.TOPK_MAX_N
 
@@ -61,53 +61,42 @@ def topk_columns(rdd, P, thresholds, top_n, reverse):
     return [(k, o[0], v) for k, o, (v,) in join.partition_slices(gk.view(keys.dtype), off, [cand], pg, rows)]
 
 
-class ColumnarTopByKeyRDD(RDD):
+class ColumnarTopByKeyRDD(DeviceResultRDD):
     """The result of topByKey(top_n, reverse=...) of a numeric ColumnarRDD in a one-process job: per key its top_n
     values, the rows of groupByKey(...).mapValue(stable sort, cut), computed on the GPU the first time a partition is
     asked for and kept.  It has the group-by's partitioner, so mapValue keeps it and a later groupWith reads it as a
-    narrow dependency."""
+    narrow dependency.  columns(split) hands out CUDA tensors (keys, offsets, values): keys int64 or float64, offsets
+    int64 [keys + 1], values in the input dtype (see topk_columns); when the float values hold a NaN the composition's
+    rows stand."""
 
     def __init__(self, parent, part, top_n, reverse):
-        RDD.__init__(self, parent.ctx)
+        DeviceResultRDD.__init__(self, parent.ctx)
         self.parent = parent
         self.partitioner = part
         self.top_n, self.reverse = top_n, reverse
         self._splits = [Split(i) for i in range(part.numPartitions)]
-        self._result = None
 
     def parents(self):
         return [self.parent]
 
-    def _materialize(self):
-        """The partitions' columns, or, when the float values hold a NaN, the composition RDD whose rows stand."""
-        if self._result is None:
-            from .engine import _device
-            vals, p = self.parent.vals, self.partitioner
-            if vals.dtype.is_floating_point and bool(torch.isnan(vals.to(_device())).any()):
-                self._result = self.parent.groupByKey(p).mapValue(top_values(self.top_n, None, self.reverse))
-            else:
-                self._result = topk_columns(self.parent, p.numPartitions, p.thresholds, self.top_n, self.reverse)
-        return self._result
+    def _run(self):
+        from .engine import _device
+        vals, p = self.parent.vals, self.partitioner
+        if vals.dtype.is_floating_point and bool(torch.isnan(vals.to(_device())).any()):
+            return None
+        return topk_columns(self.parent, p.numPartitions, p.thresholds, self.top_n, self.reverse)
 
-    def columns(self, split):
-        """Extension: partition `split` as CUDA tensors (keys, offsets, values): keys int64 or float64, offsets int64
-        [keys + 1], values in the input dtype (see topk_columns)."""
-        res = self._materialize()
-        if isinstance(res, RDD):
-            from .engine import _device
-            dev = _device()
-            rows = list(res.iterator(res.splits[split.index]))
-            kdt = torch.float64 if self.parent.keys.dtype.is_floating_point else torch.int64
-            off = [0] + list(itertools.accumulate(len(vs) for _, vs in rows))
-            return (torch.tensor([k for k, _ in rows], dtype=kdt, device=dev),
-                    torch.tensor(off, dtype=torch.int64, device=dev),
-                    torch.tensor([v for _, vs in rows for v in vs], dtype=self.parent.vals.dtype, device=dev))
-        return res[split.index]
+    def _composition(self):
+        return self.parent.groupByKey(self.partitioner).mapValue(top_values(self.top_n, None, self.reverse))
 
-    def compute(self, split):
-        res = self._materialize()
-        if isinstance(res, RDD):
-            return res.iterator(res.splits[split.index])
-        keys, offsets, values = res[split.index]
+    def _columns_of_rows(self, rows, dev):
+        kdt = torch.float64 if self.parent.keys.dtype.is_floating_point else torch.int64
+        off = [0] + list(itertools.accumulate(len(vs) for _, vs in rows))
+        return (torch.tensor([k for k, _ in rows], dtype=kdt, device=dev),
+                torch.tensor(off, dtype=torch.int64, device=dev),
+                torch.tensor([v for _, vs in rows for v in vs], dtype=self.parent.vals.dtype, device=dev))
+
+    def _rows(self, columns):
+        keys, offsets, values = columns
         off, vals = offsets.cpu().tolist(), values.cpu().tolist()
         return zip(keys.cpu().tolist(), [vals[off[j]:off[j + 1]] for j in range(len(off) - 1)])
