@@ -35,6 +35,7 @@ EXPORTS = [
     "dpk_key_or", "dpk_radix_pass", "dpk_group_heads_workspace_bytes", "dpk_group_heads", "dpk_gather_i64",
     "dpk_partition_scatter_ptrs", "dpk_copy_segments", "dpk_hash_tuple", "dpk_push_plan", "dpk_push_plan_part", "dpk_pipe_plan", "dpk_fused_plan", "dpk_memcpy_batch",
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
+    "dpk_tokenize_utf8_count", "dpk_tokenize_utf8_emit",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
     "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
@@ -84,6 +85,8 @@ def lib():
         L.dpk_tokenize_blocks.argtypes = [i64]
         L.dpk_tokenize_count.argtypes = [vp, i64, vp, vp, vp]
         L.dpk_tokenize_emit.argtypes = [vp, i64, vp, vp, vp, vp]
+        L.dpk_tokenize_utf8_count.argtypes = [vp, i64, vp, vp, vp]
+        L.dpk_tokenize_utf8_emit.argtypes = [vp, i64, vp, vp, vp, vp]
         L.dpk_gather_bytes.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp]
         L.dpk_combine_workspace_bytes.argtypes = [i64, i32, i32]
         L.dpk_combine.argtypes = [vp, ci, vp, vp, ci, i64, ci, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp,
@@ -535,6 +538,34 @@ def tokenize(data):
     lens = torch.empty(total, dtype=torch.int64, device=dev)
     if total:
         _check(lib().dpk_tokenize_emit(_ptr(data), n, _ptr(base), _ptr(starts), _ptr(lens), _stream()))
+    return starts, lens, True
+
+
+def tokenize_utf8(data):
+    """Tokens of a UTF-8 byte range on the device, as str.split() without arguments finds them in the decoded text
+    (Unicode whitespace): (starts, lens, valid) -- int64 device tensors in text order, each token given by the
+    (start, length) of its bytes; valid False = the range is not strict UTF-8, bytes.decode("utf-8") raises on it
+    (starts / lens are None then).  One host read, as tokenize."""
+    _need_cuda(data)
+    n = int(data.numel())
+    dev = data.device
+    if n == 0:
+        z = torch.zeros(0, dtype=torch.int64, device=dev)
+        return z, z.clone(), True
+    nb = int(lib().dpk_tokenize_blocks(n))
+    counts = torch.empty(nb + 1, dtype=torch.int64, device=dev)   # [nb] = the ill-formed flag
+    counts[nb] = 0
+    _check(lib().dpk_tokenize_utf8_count(_ptr(data), n, _ptr(counts), C.c_void_p(counts.data_ptr() + 8 * nb),
+                                         _stream()))
+    incl = torch.cumsum(counts[:nb], 0)
+    total, flag = int(incl[-1].item()), int(counts[nb].item())
+    if flag & 1:
+        return None, None, False
+    base = (incl - counts[:nb]).contiguous()
+    starts = torch.empty(total, dtype=torch.int64, device=dev)
+    lens = torch.empty(total, dtype=torch.int64, device=dev)
+    if total:
+        _check(lib().dpk_tokenize_utf8_emit(_ptr(data), n, _ptr(base), _ptr(starts), _ptr(lens), _stream()))
     return starts, lens, True
 
 

@@ -844,5 +844,101 @@ __host__ __device__ __forceinline__ uint32_t tok_starts16(const uint8_t *__restr
     return m;
 }
 
+// ------------------------------------------------------------- f4: UTF-8 tokeniser arithmetic (dpk_strings.cu k_tok8_*)
+// str.split() without arguments on text decoded with strict utf-8: whitespace = the code points c with
+// chr(c).isspace(): U+0009..000D, U+001C..0020, U+0085, U+00A0, U+1680, U+2000..200A, U+2028, U+2029, U+202F, U+205F,
+// U+3000 -- UTF-8 forms of 1, 2 or 3 bytes, each beginning with a lead byte, so none matches from the middle of
+// another code point.  A token = a maximal run of non-whitespace code points.
+
+// length of the whitespace code point whose UTF-8 form begins c0 c1 c2; 0: the code point there is not whitespace
+__host__ __device__ __forceinline__ int tok8_ws(uint32_t c0, uint32_t c1, uint32_t c2) {
+    if (c0 < 0x80) return tok_ws((uint8_t)c0) ? 1 : 0;
+    if (c0 == 0xC2) return (c1 == 0x85 || c1 == 0xA0) ? 2 : 0;                   // U+0085, U+00A0
+    const uint32_t v = (c0 << 16) | (c1 << 8) | c2;
+    const bool w = v == 0xE19A80u || v == 0xE38080u                               // U+1680, U+3000
+                   || (v >= 0xE28080u && v <= 0xE2808Au)                         // U+2000..200A
+                   || v == 0xE280A8u || v == 0xE280A9u || v == 0xE280AFu || v == 0xE2819Fu;   // U+2028 2029 202F 205F
+    return w ? 3 : 0;
+}
+
+// is a whitespace code point's form at data[i] (bytes past n read as 0x00, which matches none)
+__host__ __device__ __forceinline__ bool tok8_ws_at(const uint8_t *__restrict__ data, int64_t n, int64_t i) {
+    const uint32_t c0 = data[i];
+    if (c0 < 0x80) return tok_ws((uint8_t)c0);
+    const uint32_t c1 = i + 1 < n ? data[i + 1] : 0u, c2 = i + 2 < n ? data[i + 2] : 0u;
+    return tok8_ws(c0, c1, c2) != 0;
+}
+
+// the sequence length a byte announces: 1 ASCII, 0 continuation (10xxxxxx), 2 / 3 / 4 by its high bits
+__host__ __device__ __forceinline__ int tok8_len(uint32_t c) { return c < 0x80 ? 1 : c < 0xC0 ? 0 : c < 0xE0 ? 2 : c < 0xF0 ? 3 : 4; }
+
+// strict UTF-8 (Unicode Table 3-7, what bytes.decode("utf-8") accepts): does the lead byte c0 begin a well-formed
+// sequence with the bytes c1 c2 c3 after it?  Rejects C0, C1 and F5..FF, overlong 3- and 4-byte forms (E0 80..9F,
+// F0 80..8F), surrogates (ED A0..BF), values above U+10FFFF (F4 90..BF) and a missing continuation byte.
+__host__ __device__ __forceinline__ bool tok8_seq_ok(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3) {
+    const bool k2 = (c2 & 0xC0u) == 0x80u, k3 = (c3 & 0xC0u) == 0x80u;
+    const uint32_t lo = c0 == 0xE0 ? 0xA0u : c0 == 0xF0 ? 0x90u : 0x80u;          // second byte's range
+    const uint32_t hi = c0 == 0xED ? 0x9Fu : c0 == 0xF4 ? 0x8Fu : 0xBFu;
+    const bool k1 = c1 >= lo && c1 <= hi;
+    if (c0 < 0x80) return true;
+    if (c0 < 0xC2) return false;                                                   // continuation, or overlong C0 / C1
+    if (c0 < 0xE0) return k1;
+    if (c0 < 0xF0) return k1 && k2;
+    if (c0 < 0xF5) return k1 && k2 && k3;
+    return false;
+}
+
+// The per-thread step of k_tok8_count / k_tok8_emit over data[i0, i0 + 16): bit j of the result = a token starts at
+// byte i0 + j (a non-whitespace code point's lead byte after a whitespace code point or at byte 0); *bad = some byte
+// of the slice is ill-formed: a lead byte that does not begin a well-formed sequence inside [0, n), or a
+// continuation byte that no lead byte at most 3 bytes before it announces (with every lead byte checked, that is a
+// continuation byte outside any sequence).  Reads 3 bytes before the slice (the whitespace code point that may end
+// just before it, the lead of a sequence running into it) and 3 after (the sequences that begin in it).
+__host__ __device__ __forceinline__ uint32_t tok8_starts16(const uint8_t *__restrict__ data, int64_t n, int64_t i0, bool *bad) {
+    uint8_t c[3 + TK_BYTES + 3];                     // c[k] = data[i0 - 3 + k], 0x00 outside [0, n)
+    if (i0 >= 4 && i0 + TK_BYTES + 4 <= n && (((uintptr_t)(data + i0)) & 15u) == 0) {
+        const uint32_t b = *reinterpret_cast<const uint32_t *>(data + i0 - 4);
+        const uint4 q = *reinterpret_cast<const uint4 *>(data + i0);
+        const uint32_t a = *reinterpret_cast<const uint32_t *>(data + i0 + TK_BYTES);
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int k = 0; k < 3; k++) c[k] = (uint8_t)(b >> ((k + 1) * 8));
+#pragma unroll
+        for (int j = 0; j < TK_BYTES; j++) c[3 + j] = (uint8_t)(w[j >> 2] >> ((j & 3) * 8));
+#pragma unroll
+        for (int k = 0; k < 3; k++) c[3 + TK_BYTES + k] = (uint8_t)(a >> (k * 8));
+    } else {
+#pragma unroll
+        for (int k = 0; k < 3 + TK_BYTES + 3; k++) {
+            const int64_t i = i0 - 3 + k;
+            c[k] = i >= 0 && i < n ? data[i] : (uint8_t)0;
+        }
+    }
+    // l1 / l2 / l3: tok8_ws at the 1st / 2nd / 3rd byte before the current one; a whitespace code point ends just
+    // before byte j exactly when l1 == 1, l2 == 2 or l3 == 3
+    int l3 = tok8_ws(c[0], c[1], c[2]), l2 = tok8_ws(c[1], c[2], c[3]), l1 = tok8_ws(c[2], c[3], c[4]);
+    uint32_t m = 0;
+    bool b = false;
+#pragma unroll
+    for (int j = 0; j < TK_BYTES; j++) {
+        const int k = 3 + j;
+        const int l0 = tok8_ws(c[k], c[k + 1], c[k + 2]);
+        if (i0 + j < n) {
+            const bool lead = (c[k] & 0xC0u) != 0x80u;
+            if (lead) {
+                b |= !tok8_seq_ok(c[k], c[k + 1], c[k + 2], c[k + 3]);
+                if (l0 == 0 && (i0 + j == 0 || l1 == 1 || l2 == 2 || l3 == 3)) m |= 1u << j;
+            } else {
+                b |= !(tok8_len(c[k - 1]) >= 2 || tok8_len(c[k - 2]) >= 3 || tok8_len(c[k - 3]) >= 4);
+            }
+        }
+        l3 = l2;
+        l2 = l1;
+        l1 = l0;
+    }
+    *bad = b;
+    return m;
+}
+
 
 }  // namespace dpk

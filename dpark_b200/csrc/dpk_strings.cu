@@ -104,6 +104,61 @@ k_tok_emit(const uint8_t *__restrict__ data, int64_t n, const int64_t *__restric
     }
 }
 
+// The same two passes for UTF-8 text (the ranges the ASCII pair declines): TextFileRDD decodes every line with strict
+// utf-8, so a range is either well-formed as a whole ('\n' never occurs inside a multi-byte sequence) or the row-wise
+// path raises UnicodeDecodeError; whitespace is every code point str.isspace() accepts, 1 to 3 bytes long.
+// tok8_starts16 (dpk_common.cuh) classifies the lead bytes of a 16-byte slice and checks their sequences; any
+// ill-formed byte raises `flags` bit 0, and the caller then runs no emit.  The emit walks each token to the lead byte of
+// the next whitespace code point.
+__global__ void __launch_bounds__(TK_THREADS)
+k_tok8_count(const uint8_t *__restrict__ data, int64_t n, int64_t *__restrict__ block_counts, unsigned long long *__restrict__ flags) {
+    __shared__ int s_w[TK_THREADS / 32];
+    const int64_t i0 = ((int64_t)blockIdx.x * TK_THREADS + threadIdx.x) * TK_BYTES;
+    bool bad = false;
+    const uint32_t m = i0 < n ? tok8_starts16(data, n, i0, &bad) : 0u;
+    int c = __popc(m);
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = c;
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(flags, 1ull);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int w = 0; w < TK_THREADS / 32; w++) t += s_w[w];
+        block_counts[blockIdx.x] = t;
+    }
+}
+
+__global__ void __launch_bounds__(TK_THREADS)
+k_tok8_emit(const uint8_t *__restrict__ data, int64_t n, const int64_t *__restrict__ block_base, int64_t *__restrict__ starts,
+            int64_t *__restrict__ lens) {
+    __shared__ int s_w[TK_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t i0 = ((int64_t)blockIdx.x * TK_THREADS + threadIdx.x) * TK_BYTES;
+    bool bad = false;
+    uint32_t m = i0 < n ? tok8_starts16(data, n, i0, &bad) : 0u;
+    const int c = __popc(m);
+    int incl = c;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    int before = 0;
+    for (int w = 0; w < warp; w++) before += s_w[w];
+    int64_t r = block_base[blockIdx.x] + before + incl - c;
+    while (m) {
+        const int j = __ffs(m) - 1;
+        m &= m - 1;
+        const int64_t b = i0 + j;
+        int64_t e = b + 1;
+        while (e < n && !tok8_ws_at(data, n, e)) e++;
+        starts[r] = b;
+        lens[r] = e - b;
+        r++;
+    }
+}
+
 // out[out_off[i] .. out_off[i] + lens[row]) = data[starts[row] ..), row = idx ? idx[i] : i  (token bytes made contiguous:
 // the (data, offsets) form dpk_hash_bytes / dpk_dict_encode take; or the bytes of the distinct keys for the host)
 __global__ void __launch_bounds__(256)
@@ -154,6 +209,29 @@ int dpk_tokenize_emit(const uint8_t *data, int64_t n, const int64_t *block_base,
     if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
     cudaStream_t st = (cudaStream_t)stream;
     DPK_LAUNCH("tok_emit", st, k_tok_emit<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_base, starts, lens));
+    return DPK_OK;
+}
+
+int dpk_tokenize_utf8_count(const uint8_t *data, int64_t n, int64_t *block_counts, int64_t *flags, dpk_stream_t stream) {
+    if (n < 0) return fail(DPK_ERR_INVALID, "n=%lld < 0", (long long)n);
+    if (n == 0) return DPK_OK;
+    if (!data || !block_counts || !flags) return fail(DPK_ERR_INVALID, "NULL pointer");
+    const int64_t nb = dpk_tokenize_blocks(n);
+    if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
+    cudaStream_t st = (cudaStream_t)stream;
+    DPK_LAUNCH("tok8_count", st, k_tok8_count<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_counts, (unsigned long long *)flags));
+    return DPK_OK;
+}
+
+int dpk_tokenize_utf8_emit(const uint8_t *data, int64_t n, const int64_t *block_base, int64_t *starts, int64_t *lens,
+                           dpk_stream_t stream) {
+    if (n < 0) return fail(DPK_ERR_INVALID, "n=%lld < 0", (long long)n);
+    if (n == 0) return DPK_OK;
+    if (!data || !block_base || !starts || !lens) return fail(DPK_ERR_INVALID, "NULL pointer");
+    const int64_t nb = dpk_tokenize_blocks(n);
+    if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
+    cudaStream_t st = (cudaStream_t)stream;
+    DPK_LAUNCH("tok8_emit", st, k_tok8_emit<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_base, starts, lens));
     return DPK_OK;
 }
 

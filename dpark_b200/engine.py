@@ -65,8 +65,11 @@ def run_shuffle(srdd):
     if srdd.kind == "reduce":
         from . import textingest
         text = textingest.recognize(srdd.parent) if TEXT_INGEST else None
-        if text is not None:     # the word-count shape: tokenise on the device (None back: a non-ASCII split, row-wise path)
+        if text is not None:     # the word-count shape: tokenise on the device (ASCII first, then UTF-8; None back from
+            # both: the text is not strict UTF-8 and the row-wise path raises the reference's UnicodeDecodeError)
             res = textingest.reduce_tokens(text, range(len(text.splits)), P, thr, srdd.op, dev, ShuffleResult(P))
+            if res is None:
+                res = textingest.reduce_tokens_utf8(text, range(len(text.splits)), P, thr, srdd.op, dev, ShuffleResult(P))
             if res is not None:
                 return res
         splits = _gather_parent(srdd, True)
@@ -121,6 +124,8 @@ def _run_shuffle_spmd(srdd, rank, world):
         text = textingest.recognize(srdd.parent)
         if text is not None:
             part = textingest.reduce_tokens(text, sorted(mine), P, thr, srdd.op, dev, ShuffleResult(P))
+            if part is None:
+                part = textingest.reduce_tokens_utf8(text, sorted(mine), P, thr, srdd.op, dev, ShuffleResult(P))
             if part is not None:
                 ks = [k for p in range(P) for k in part.parts[p][0]]
                 vs = [v for p in range(P) for v in part.parts[p][1]]

@@ -6,14 +6,20 @@ In the reference -- and on this package's row-wise path -- every line is decoded
 function and every token becomes a (str, int) tuple before the shuffle sees it: the end-to-end time of BASELINE config 1
 is that interpreter loop (scripts/wc_e2e.py <lines> rowwise times it).  When the functions between
 `textFile` and the shuffle are, byte code for byte code, one of the tokenising shapes below, the same rows are produced
-on the GPU instead: the file's bytes go to HBM, `dpk_tokenize_*` finds the tokens (str.split() semantics for ASCII
-text), and the token bytes feed the existing variable-length-key shuffle (dpk_hash_bytes -> dpk_dict_encode ->
-dpk_partition -> dpk_combine).  Only the distinct words and their counts come back.
+on the GPU instead: the file's bytes go to HBM, `dpk_tokenize_*` finds the tokens (str.split() semantics), and the
+token bytes feed the existing variable-length-key shuffle (dpk_hash_bytes -> dpk_dict_encode -> dpk_partition ->
+dpk_combine).  Only the distinct words and their counts come back.
+
+Two tokenisers, tried in this order: `reduce_tokens` (dpk_tokenize_count / _emit) takes text that is ASCII throughout
+and declines at the first piece holding a byte >= 0x80; `reduce_tokens_utf8` (dpk_tokenize_utf8_count / _emit) then
+runs the whole job again over UTF-8 text, with Python's Unicode whitespace (every code point c with chr(c).isspace(),
+separators of 1 to 3 bytes) and strict decoding.  TextFileRDD decodes every line with strict utf-8, so when a range is
+not well-formed UTF-8 the device declines the whole job and the row-wise path raises the reference's
+UnicodeDecodeError.  Keys come back as the decoded tokens, not normalised, exactly as str.split() leaves them.
 
 Recognition is structural and exact -- the user's code object must equal a template's (instructions, constants,
-attribute names, signature; no closure, no defaults) -- never a behavioural probe: anything else, any split holding a
-byte >= 0x80 (Unicode whitespace, decoding errors: Python's business), and any subclass of the RDD types involved takes
-the row-wise path unchanged.
+attribute names, signature; no closure, no defaults) -- never a behavioural probe: anything else, any split that is
+not well-formed UTF-8, and any subclass of the RDD types involved takes the row-wise path unchanged.
 """
 import os
 import types
@@ -120,6 +126,17 @@ def reduce_tokens(text_rdd, split_indices, P, thresholds, op, dev, res, local_on
     res.parts[p] = (keys, values) for every partition and returns res; returns None (nothing done) when a split
     holds a non-ASCII byte.  The splits' owned ranges are contiguous when the indices are, and every line belongs to
     exactly one split, so consecutive splits are read as one byte range."""
+    return _reduce(text_rdd, split_indices, P, thresholds, op, dev, res, local_only, nv.tokenize, "ascii")
+
+
+def reduce_tokens_utf8(text_rdd, split_indices, P, thresholds, op, dev, res, local_only=True):
+    """reduce_tokens for UTF-8 text: the tokens are those str.split() finds in the decoded lines (Unicode whitespace),
+    the keys their `bytes.decode("utf-8")`.  Returns None (nothing done) only when a split is not strict UTF-8 -- the
+    row-wise path then raises the UnicodeDecodeError TextFileRDD.compute raises."""
+    return _reduce(text_rdd, split_indices, P, thresholds, op, dev, res, local_only, nv.tokenize_utf8, "utf-8")
+
+
+def _reduce(text_rdd, split_indices, P, thresholds, op, dev, res, local_only, tokenize, encoding):
     path = text_rdd.path
     size = os.path.getsize(path)
     splits = text_rdd.splits
@@ -135,8 +152,8 @@ def reduce_tokens(text_rdd, split_indices, P, thresholds, op, dev, res, local_on
     for a, b in [piece for r in ranges for piece in cut_pieces(path, r[0], r[1], size)]:
         host = np.fromfile(path, dtype=np.uint8, count=b - a, offset=a)
         d_text = torch.from_numpy(host).to(dev)
-        starts, lens, ascii_ok = nv.tokenize(d_text)
-        if not ascii_ok:
+        starts, lens, ok = tokenize(d_text)
+        if not ok:
             return None
         if starts.numel():
             pieces.append(nv.gather_bytes(d_text, starts, lens))
@@ -158,8 +175,8 @@ def reduce_tokens(text_rdd, split_indices, P, thresholds, op, dev, res, local_on
     if n >= (1 << 31):
         raise nv.NativeError("more than 2^31 tokens in one shuffle")
     ones = torch.ones(n, dtype=torch.int64, device=dev)
-    h = nv.hash_bytes(tok, off, nv.STR_UTF8)          # ASCII: code points == bytes (unicode_hash, portable_hash.pyx:33-48)
-    rep = nv.dict_encode(tok, off, h)
+    h = nv.hash_bytes(tok, off, nv.STR_UTF8)          # str keys hash by code point (unicode_hash, portable_hash.pyx:33-48)
+    rep = nv.dict_encode(tok, off, h)                 # strict UTF-8: equal strings are equal bytes
     sb = shuffle.choose_sub_bits(n, P)
     ctx = shuffle.local_only() if local_only else _Null()
     with ctx:
@@ -178,7 +195,7 @@ def reduce_tokens(text_rdd, split_indices, P, thresholds, op, dev, res, local_on
     at = 0
     for p in range(P):
         c = cnt_h[p]
-        keys = [raw[ko_h[i]:ko_h[i + 1]].decode("ascii") for i in range(at, at + c)]
+        keys = [raw[ko_h[i]:ko_h[i + 1]].decode(encoding) for i in range(at, at + c)]
         res.parts[p] = (keys, vals[at:at + c])
         at += c
     return res

@@ -483,6 +483,16 @@ int dpk_tokenize_emit(const uint8_t *data, int64_t n, const int64_t *block_base,
                       dpk_stream_t stream);
 int dpk_gather_bytes(const uint8_t *data, const int64_t *starts, const int64_t *lens, const int64_t *idx, int64_t m,
                      const int64_t *out_off, uint8_t *out, dpk_stream_t stream);
+/* The same pair for UTF-8 text (a range the ASCII pair declines), with the same block counts, scan and outputs.
+ * Tokens = maximal runs of code points c with !chr(c).isspace() (Python's whitespace: U+0009..000D, U+001C..0020,
+ * U+0085, U+00A0, U+1680, U+2000..200A, U+2028, U+2029, U+202F, U+205F, U+3000), each as the (start, length) of its
+ * UTF-8 bytes.  dpk_tokenize_utf8_count ORs bit 0 into *flags if the range is not strict UTF-8 (what
+ * bytes.decode("utf-8") rejects: stray continuation bytes, C0, C1, F5..FF, overlong forms, surrogates, values above
+ * U+10FFFF, a sequence cut short by the end of the range); the caller must then run no emit and leave the range to
+ * the row-wise path, which raises UnicodeDecodeError. */
+int dpk_tokenize_utf8_count(const uint8_t *data, int64_t n, int64_t *block_counts, int64_t *flags, dpk_stream_t stream);
+int dpk_tokenize_utf8_emit(const uint8_t *data, int64_t n, const int64_t *block_base, int64_t *starts, int64_t *lens,
+                           dpk_stream_t stream);
 
 /* ---- variable-length keys (str / bytes): key identity on the device ---------
  * The reference's dicts compare keys by value; two different strings may share
