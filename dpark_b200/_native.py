@@ -35,7 +35,7 @@ EXPORTS = [
     "dpk_key_or", "dpk_radix_pass", "dpk_group_heads_workspace_bytes", "dpk_group_heads", "dpk_gather_i64",
     "dpk_partition_scatter_ptrs", "dpk_copy_segments", "dpk_hash_tuple", "dpk_push_plan", "dpk_push_plan_part", "dpk_pipe_plan", "dpk_fused_plan", "dpk_memcpy_batch",
     "dpk_tokenize_blocks", "dpk_tokenize_count", "dpk_tokenize_emit", "dpk_gather_bytes",
-    "dpk_tokenize_utf8_count", "dpk_tokenize_utf8_emit",
+    "dpk_tokenize_utf8_count", "dpk_tokenize_utf8_emit", "dpk_textcols_count", "dpk_textcols_emit", "dpk_textcols_parse",
     "dpk_radix_pass_seg_workspace_bytes", "dpk_radix_pass_seg", "dpk_join_count", "dpk_join_emit",
     "dpk_cogroup_count", "dpk_cogroup_emit", "dpk_topk_lengths", "dpk_topk_round",
     "dpk_bcast_build", "dpk_bcast_probe", "dpk_bcast_emit", "dpk_sort_keys", "dpk_sort_cuts", "dpk_sort_gather",
@@ -87,6 +87,9 @@ def lib():
         L.dpk_tokenize_emit.argtypes = [vp, i64, vp, vp, vp, vp]
         L.dpk_tokenize_utf8_count.argtypes = [vp, i64, vp, vp, vp]
         L.dpk_tokenize_utf8_emit.argtypes = [vp, i64, vp, vp, vp, vp]
+        L.dpk_textcols_count.argtypes = [vp, i64, vp, vp, vp]
+        L.dpk_textcols_emit.argtypes = [vp, i64, vp, vp, vp]
+        L.dpk_textcols_parse.argtypes = [vp, i64, vp, i64, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp]
         L.dpk_gather_bytes.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp]
         L.dpk_combine_workspace_bytes.argtypes = [i64, i32, i32]
         L.dpk_combine.argtypes = [vp, ci, vp, vp, ci, i64, ci, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp,
@@ -567,6 +570,58 @@ def tokenize_utf8(data):
     if total:
         _check(lib().dpk_tokenize_utf8_emit(_ptr(data), n, _ptr(base), _ptr(starts), _ptr(lens), _stream()))
     return starts, lens, True
+
+
+def line_starts(data):
+    """Every line start of a byte range on the device (byte 0 and each byte after a '\\n', inside the range; a final
+    '\\n' opens no line): (starts int64 device tensor in text order, high) -- high True when the range holds a byte
+    >= 0x80.  One host read (the line count sizes the output)."""
+    _need_cuda(data)
+    n = int(data.numel())
+    dev = data.device
+    if n == 0:
+        return torch.zeros(0, dtype=torch.int64, device=dev), False
+    nb = int(lib().dpk_tokenize_blocks(n))
+    counts = torch.empty(nb + 1, dtype=torch.int64, device=dev)   # [nb] = the high-byte flag
+    counts[nb] = 0
+    _check(lib().dpk_textcols_count(_ptr(data), n, _ptr(counts), C.c_void_p(counts.data_ptr() + 8 * nb), _stream()))
+    incl = torch.cumsum(counts, 0)
+    total, flag = int(incl[nb - 1].item()), int(counts[nb].item())
+    base = (incl[:nb] - counts[:nb]).contiguous()
+    starts = torch.empty(total, dtype=torch.int64, device=dev)
+    _check(lib().dpk_textcols_emit(_ptr(data), n, _ptr(base), _ptr(starts), _stream()))
+    return starts, bool(flag & 1)
+
+
+def utf8_valid(data):
+    """Is the device byte range strict UTF-8 (what bytes.decode("utf-8") accepts)?  dpk_tokenize_utf8_count's flag."""
+    _need_cuda(data)
+    n = int(data.numel())
+    if n == 0:
+        return True
+    nb = int(lib().dpk_tokenize_blocks(n))
+    counts = torch.zeros(nb + 1, dtype=torch.int64, device=data.device)
+    _check(lib().dpk_tokenize_utf8_count(_ptr(data), n, _ptr(counts), C.c_void_p(counts.data_ptr() + 8 * nb),
+                                         _stream()))
+    return not (int(counts[nb].item()) & 1)
+
+
+def textcols_parse(data, starts, sep, key, value, key_float, value_float, out_keys=None, out_vals=None, host=None):
+    """Fields `key` and `value` of every line of the device byte range (starts from line_starts), parsed as int() or
+    float() (dpk_textcols_parse): (keys int64, vals int64, host uint8) device tensors -- float columns hold the float64
+    bits -- with host[i] = 1 where Python must parse line i.  sep: None (str.split()) or the separator's UTF-8 bytes as
+    a uint8 device tensor."""
+    _need_cuda(data, starts, sep)
+    m = int(starts.numel())
+    dev = data.device
+    out_keys = torch.empty(m, dtype=torch.int64, device=dev) if out_keys is None else out_keys
+    out_vals = torch.empty(m, dtype=torch.int64, device=dev) if out_vals is None else out_vals
+    host = torch.empty(m, dtype=torch.uint8, device=dev) if host is None else host
+    kinds = (K_F64 if key_float else K_I64, K_F64 if value_float else K_I64)
+    _check(lib().dpk_textcols_parse(_ptr(data), int(data.numel()), _ptr(starts), m, _ptr(sep),
+                                    0 if sep is None else int(sep.numel()), key, value, kinds[0], kinds[1],
+                                    _ptr(out_keys), _ptr(out_vals), _ptr(host), _stream()))
+    return out_keys, out_vals, host
 
 
 def gather_bytes(data, starts, lens, idx=None):

@@ -181,6 +181,17 @@ class DparkContext(object):
             return self.union([cls(self, p, *ka, **kws) for p in paths])
         return cls(self, path, *ka, **kws)
 
+    def textFileColumns(self, path, key=0, value=1, types=(int, int), sep=None, ext="", followLink=True, maxdepth=0,
+                        numSplits=None, splitSize=None):
+        """Extension: a ColumnarRDD of two numeric fields per line, parsed on the GPU -- split i holds the rows split i
+        of textFile(path, ext, followLink, maxdepth, numSplits=..., splitSize=...).map(parse) yields, with
+        parse(line) = (types[0](f[key]), types[1](f[value])) for f = line.split(sep).  types: int (int64 column) or
+        float (float64).  Built, and its errors raised, here (dpark_b200/textcolumns.py)."""
+        self.init()
+        from . import textcolumns
+        return textcolumns.text_file_columns(self, path, key, value, types, sep, ext, followLink, maxdepth,
+                                             numSplits, splitSize)
+
     def union(self, rdds):
         return UnionRDD(self, rdds)
 

@@ -940,5 +940,271 @@ __host__ __device__ __forceinline__ uint32_t tok8_starts16(const uint8_t *__rest
     return m;
 }
 
+// ------------------------------------------------------------- f10: numeric text columns (dpk_strings.cu k_tc_*;
+// tests/numparsecheck.cu runs the same arithmetic on the CPU).  Every line either gets its final values here or is
+// marked for the host, which runs Python's own line.split(sep) / int() / float() on it.  Accepted (ASCII only, after
+// stripping \t \n \v \f \r and space -- what int() and float() strip; \x1c..\x1f they do not):
+//   int   [+-]?[0-9]{1,19} whose value fits int64
+//   float [+-]? digits with at most one '.' and at least one digit, then optionally [eE][+-]?[0-9]+; or inf, infinity,
+//         nan in any case
+// Everything else -- '_', a byte >= 0x80, more digits, a malformed or missing field -- goes to the host.
+
+// bit j of the result: a line starts at byte i0 + j (byte 0, or the byte after a '\n', inside [0, n)); *hi |= any
+// byte of the slice >= 0x80
+__host__ __device__ __forceinline__ uint32_t tc_starts16(const uint8_t *__restrict__ data, int64_t n, int64_t i0, bool *hi) {
+    uint8_t c[TK_BYTES];
+    if (i0 + TK_BYTES <= n && (((uintptr_t)(data + i0)) & 15u) == 0) {
+        const uint4 q = *reinterpret_cast<const uint4 *>(data + i0);
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int j = 0; j < TK_BYTES; j++) c[j] = (uint8_t)(w[j >> 2] >> ((j & 3) * 8));
+    } else {
+#pragma unroll
+        for (int j = 0; j < TK_BYTES; j++) c[j] = i0 + j < n ? data[i0 + j] : (uint8_t)0;
+    }
+    bool after_nl = i0 == 0 || data[i0 - 1] == '\n';
+    uint32_t m = 0;
+    bool h = false;
+#pragma unroll
+    for (int j = 0; j < TK_BYTES; j++) {
+        if (after_nl && i0 + j < n) m |= 1u << j;
+        after_nl = c[j] == '\n';
+        h |= c[j] >= 0x80;
+    }
+    *hi = h;
+    return m;
+}
+
+// what int() and float() strip among ASCII bytes
+__host__ __device__ __forceinline__ bool tc_space(uint32_t c) { return c == 0x20 || (c >= 0x09 && c <= 0x0d); }
+
+__host__ __device__ __forceinline__ bool tc_digit(uint32_t c) { return c - '0' < 10u; }
+
+__host__ __device__ __forceinline__ uint64_t tc_ld(const uint64_t *p) {
+#ifdef __CUDA_ARCH__
+    return __ldg(reinterpret_cast<const unsigned long long *>(p));
+#else
+    return *p;
+#endif
+}
+
+__host__ __device__ __forceinline__ int tc_clz64(uint64_t x) {
+#ifdef __CUDA_ARCH__
+    return __clzll((long long)x);
+#else
+    return __builtin_clzll(x);
+#endif
+}
+
+__host__ __device__ __forceinline__ void tc_mul128(uint64_t a, uint64_t b, uint64_t *hi, uint64_t *lo) {
+#ifdef __CUDA_ARCH__
+    *hi = __umul64hi(a, b);
+    *lo = a * b;
+#else
+    const unsigned __int128 p = (unsigned __int128)a * b;
+    *hi = (uint64_t)(p >> 64);
+    *lo = (uint64_t)p;
+#endif
+}
+
+// [*b, *e) without the strippable bytes at either end
+__host__ __device__ __forceinline__ void tc_trim(const uint8_t *__restrict__ s, int64_t *b, int64_t *e) {
+    while (*b < *e && tc_space(s[*b])) ++*b;
+    while (*e > *b && tc_space(s[*e - 1])) --*e;
+}
+
+// int(s[b, e)) when the device grammar accepts it and the value fits int64
+__host__ __device__ __forceinline__ bool tc_parse_i64(const uint8_t *__restrict__ s, int64_t b, int64_t e, int64_t *out) {
+    tc_trim(s, &b, &e);
+    bool neg = false;
+    if (b < e && (s[b] == '+' || s[b] == '-')) neg = s[b++] == '-';
+    if (e - b < 1 || e - b > 19) return false;
+    uint64_t v = 0;                                  // 19 digits stay below 2^64
+    for (int64_t p = b; p < e; p++) {
+        const uint32_t d = (uint32_t)s[p] - '0';
+        if (d >= 10u) return false;
+        v = v * 10 + d;
+    }
+    if (v > (neg ? (1ull << 63) : (1ull << 63) - 1)) return false;
+    *out = (int64_t)(neg ? 0 - v : v);
+    return true;
+}
+
+// Eisel-Lemire (Lemire 2021, "Number parsing at a gigabyte per second", section 5): the binary64 bits (sign clear)
+// nearest to w * 10^q, w != 0 a 64-bit decimal significand.  pow5 = dpk_pow5.inc (2 words per q in [-342, 308]).
+// False: the truncated 128-bit product cannot decide the rounding.
+__host__ __device__ __forceinline__ bool tc_eisel_lemire(int64_t q, uint64_t w, const uint64_t *__restrict__ pow5,
+                                                         uint64_t *bits) {
+    if (q < -342) { *bits = 0; return true; }
+    if (q > 308) { *bits = 0x7FF0000000000000ull; return true; }
+    const int lz = tc_clz64(w);
+    w <<= lz;
+    const int idx = 2 * (int)(q + 342);
+    uint64_t hi, lo;
+    tc_mul128(w, tc_ld(pow5 + idx), &hi, &lo);
+    if ((hi & 0x1FF) == 0x1FF) {                     // the 9 bits below the 55 kept are all ones: refine
+        uint64_t hi2, lo2;
+        tc_mul128(w, tc_ld(pow5 + idx + 1), &hi2, &lo2);
+        lo += hi2;
+        if (hi2 > lo) hi++;
+        if ((hi & 0x1FF) == 0x1FF && lo == ~0ull) return false;   // the product's error could still carry into hi
+    }
+    const int upper = (int)(hi >> 63);
+    const int shift = upper + 9;
+    uint64_t m = hi >> shift;
+    int32_t p2 = (int32_t)(((217706 * (int32_t)q) >> 16) + 63) + upper - lz + 1023;   // floor(q log2(10)) + 63 + ...
+    if (p2 <= 0) {                                   // subnormal, or below the least subnormal
+        if (-p2 + 1 >= 64) { *bits = 0; return true; }
+        m >>= -p2 + 1;
+        m += m & 1;
+        m >>= 1;
+        *bits = m | ((uint64_t)(m < (1ull << 52) ? 0 : 1) << 52);
+        return true;
+    }
+    // an exact halfway case can only occur for q in [-4, 23]: round it to even
+    if (lo <= 1 && q >= -4 && q <= 23 && (m & 3) == 1 && (m << shift) == hi) m &= ~1ull;
+    m += m & 1;
+    m >>= 1;
+    if (m >= (2ull << 52)) { m = 1ull << 52; p2++; }
+    m &= ~(1ull << 52);
+    if (p2 >= 0x7FF) { *bits = 0x7FF0000000000000ull; return true; }
+    *bits = m | ((uint64_t)p2 << 52);
+    return true;
+}
+
+// does s[b, e) spell `word` (lower case) in any case
+__host__ __device__ __forceinline__ bool tc_word(const uint8_t *__restrict__ s, int64_t b, int64_t e, const char *word, int len) {
+    if (e - b != len) return false;
+    for (int k = 0; k < len; k++)
+        if ((s[b + k] | 0x20) != (uint8_t)word[k]) return false;
+    return true;
+}
+
+// the bits of float(s[b, e)) when the device grammar accepts it and the conversion can decide its rounding
+__host__ __device__ __forceinline__ bool tc_parse_f64(const uint8_t *__restrict__ s, int64_t b, int64_t e,
+                                                      const uint64_t *__restrict__ pow5, uint64_t *out) {
+    tc_trim(s, &b, &e);
+    uint64_t sign = 0;
+    if (b < e && (s[b] == '+' || s[b] == '-')) sign = s[b++] == '-' ? 1ull << 63 : 0;
+    if (b >= e) return false;
+    if ((s[b] | 0x20) == 'i' || (s[b] | 0x20) == 'n') {
+        if (tc_word(s, b, e, "inf", 3) || tc_word(s, b, e, "infinity", 8)) { *out = sign | 0x7FF0000000000000ull; return true; }
+        if (tc_word(s, b, e, "nan", 3)) { *out = sign | 0x7FF8000000000000ull; return true; }
+        return false;
+    }
+    // w = the first 19 significant digits, q = the decimal exponent of its last one; dropped = a nonzero digit
+    // past those 19
+    uint64_t w = 0;
+    int nd = 0;
+    int64_t q = 0;
+    bool dropped = false, any = false;
+    for (; b < e && tc_digit(s[b]); b++) {
+        const uint32_t d = s[b] - '0';
+        any = true;
+        if (nd == 0 && d == 0) continue;
+        if (nd < 19) { w = w * 10 + d; nd++; } else { q++; dropped |= d != 0; }
+    }
+    if (b < e && s[b] == '.') {
+        for (b++; b < e && tc_digit(s[b]); b++) {
+            const uint32_t d = s[b] - '0';
+            any = true;
+            if (nd == 0 && d == 0) { q--; continue; }
+            if (nd < 19) { w = w * 10 + d; nd++; q--; } else { dropped |= d != 0; }
+        }
+    }
+    if (!any) return false;
+    if (b < e && (s[b] | 0x20) == 'e') {
+        b++;
+        bool eneg = false;
+        if (b < e && (s[b] == '+' || s[b] == '-')) eneg = s[b++] == '-';
+        if (b >= e || !tc_digit(s[b])) return false;
+        int64_t x = 0;
+        for (; b < e && tc_digit(s[b]); b++) x = x < 1000000000000ll ? x * 10 + (s[b] - '0') : x;   // saturates far
+        q += eneg ? -x : x;                                                                           // outside 10^308
+    }
+    if (b != e) return false;
+    if (w == 0) { *out = sign; return true; }
+    if (!dropped && q >= -22 && q <= 22 && w <= (1ull << 53)) {       // exact operands, one correctly rounded op
+        double p = 1.0;
+        for (int64_t k = q < 0 ? -q : q; k > 0; k--) p *= 10.0;        // 10^k, k <= 22, is exact
+        const double v = q < 0 ? (double)w / p : (double)w * p;
+        uint64_t vb;
+        memcpy(&vb, &v, 8);
+        *out = sign | vb;
+        return true;
+    }
+    uint64_t lo;
+    if (!tc_eisel_lemire(q, w, pow5, &lo)) return false;
+    if (dropped) {                                   // the value lies in (w, w + 1) * 10^q: both ends must agree
+        uint64_t hi;
+        if (!tc_eisel_lemire(q, w + 1, pow5, &hi) || hi != lo) return false;
+    }
+    *out = sign | lo;
+    return true;
+}
+
+// The fields k0 and k1 of the line s[b, e) as [f[0], f[1]) and [f[2], f[3]): line.split() (sep_len == 0: maximal runs
+// of non-whitespace code points, tok8_ws) or line.split(sep) (the matches of sep[0, sep_len) from left to right,
+// without overlap).  Walks no further than field max(k0, k1); false when the line has fewer fields.
+__host__ __device__ __forceinline__ int tc_ws_len(const uint8_t *__restrict__ s, int64_t p, int64_t e) {
+    const uint32_t c0 = s[p];
+    if (c0 < 0x80) return tok_ws((uint8_t)c0) ? 1 : 0;
+    return tok8_ws(c0, p + 1 < e ? s[p + 1] : 0u, p + 2 < e ? s[p + 2] : 0u);
+}
+
+__host__ __device__ __forceinline__ bool tc_fields(const uint8_t *__restrict__ s, int64_t b, int64_t e,
+                                                   const uint8_t *__restrict__ sep, int32_t sep_len, int32_t k0,
+                                                   int32_t k1, int64_t *f) {
+    const int32_t last = k0 > k1 ? k0 : k1;
+    int64_t p = b;
+    for (int32_t fi = 0;; fi++) {
+        int64_t fb, fe;
+        bool more;
+        if (sep_len == 0) {
+            for (int l; p < e && (l = tc_ws_len(s, p, e)) != 0;) p += l;
+            if (p >= e) return false;
+            fb = p;
+            while (p < e && tc_ws_len(s, p, e) == 0) p++;
+            fe = p;
+            more = true;
+        } else {
+            fb = p;
+            const uint8_t s0 = sep[0];
+            for (; p + sep_len <= e; p++) {
+                if (s[p] != s0) continue;
+                int32_t k = 1;
+                while (k < sep_len && s[p + k] == sep[k]) k++;
+                if (k == sep_len) break;
+            }
+            more = p + sep_len <= e;
+            fe = more ? p : e;
+            p = more ? p + sep_len : e;
+        }
+        if (fi == k0) { f[0] = fb; f[1] = fe; }
+        if (fi == k1) { f[2] = fb; f[3] = fe; }
+        if (fi == last) return true;
+        if (!more) return false;
+    }
+}
+
+// one line s[b, e): its key and value (int64 or float64 bits by kind DPK_K_I64 / DPK_K_F64); false = a host line
+__host__ __device__ __forceinline__ bool tc_parse_field(const uint8_t *__restrict__ s, int64_t b, int64_t e, int32_t kind,
+                                                        const uint64_t *__restrict__ pow5, int64_t *out) {
+    if (kind == DPK_K_I64) return tc_parse_i64(s, b, e, out);
+    uint64_t bits;
+    if (!tc_parse_f64(s, b, e, pow5, &bits)) return false;
+    *out = (int64_t)bits;
+    return true;
+}
+
+__host__ __device__ __forceinline__ bool tc_line(const uint8_t *__restrict__ s, int64_t b, int64_t e,
+                                                 const uint8_t *__restrict__ sep, int32_t sep_len, int32_t key,
+                                                 int32_t value, int32_t key_kind, int32_t value_kind,
+                                                 const uint64_t *__restrict__ pow5, int64_t *k, int64_t *v) {
+    int64_t f[4];
+    return tc_fields(s, b, e, sep, sep_len, key, value, f) && tc_parse_field(s, f[0], f[1], key_kind, pow5, k)
+           && tc_parse_field(s, f[2], f[3], value_kind, pow5, v);
+}
+
 
 }  // namespace dpk

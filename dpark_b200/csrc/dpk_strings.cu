@@ -159,6 +159,76 @@ k_tok8_emit(const uint8_t *__restrict__ data, int64_t n, const int64_t *__restri
     }
 }
 
+// ---- numeric text columns (textFileColumns) ----------------------------------------------------------------------------
+// k_tc_count / k_tc_emit: the line starts of a byte range in the tokenisers' layout (16 bytes per thread, 4096-byte
+// blocks, block counts, the host-side scan, then every start in text order); the count pass also ORs bit 0 into
+// `flags` when a byte >= 0x80 occurs, so that the UTF-8 check runs only on such ranges.  k_tc_parse: one thread per
+// line finds the key and value fields and parses them (tc_line, dpk_common.cuh), or marks the line for the host.
+// The powers of five live in global memory and are read through L1: lanes index them divergently.
+__device__ const uint64_t g_tc_pow5[] = {
+#include "dpk_pow5.inc"
+};
+
+__global__ void __launch_bounds__(TK_THREADS)
+k_tc_count(const uint8_t *__restrict__ data, int64_t n, int64_t *__restrict__ block_counts, unsigned long long *__restrict__ flags) {
+    __shared__ int s_w[TK_THREADS / 32];
+    const int64_t i0 = ((int64_t)blockIdx.x * TK_THREADS + threadIdx.x) * TK_BYTES;
+    bool hi = false;
+    const uint32_t m = i0 < n ? tc_starts16(data, n, i0, &hi) : 0u;
+    int c = __popc(m);
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = c;
+    if (__any_sync(0xffffffffu, hi) && (threadIdx.x & 31) == 0) atomicOr(flags, 1ull);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int w = 0; w < TK_THREADS / 32; w++) t += s_w[w];
+        block_counts[blockIdx.x] = t;
+    }
+}
+
+__global__ void __launch_bounds__(TK_THREADS)
+k_tc_emit(const uint8_t *__restrict__ data, int64_t n, const int64_t *__restrict__ block_base, int64_t *__restrict__ starts) {
+    __shared__ int s_w[TK_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t i0 = ((int64_t)blockIdx.x * TK_THREADS + threadIdx.x) * TK_BYTES;
+    bool hi = false;
+    uint32_t m = i0 < n ? tc_starts16(data, n, i0, &hi) : 0u;
+    const int c = __popc(m);
+    int incl = c;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    int before = 0;
+    for (int w = 0; w < warp; w++) before += s_w[w];
+    int64_t r = block_base[blockIdx.x] + before + incl - c;
+    while (m) {
+        const int j = __ffs(m) - 1;
+        m &= m - 1;
+        starts[r++] = i0 + j;
+    }
+}
+
+// line i = data[starts[i], the next '\n' or n); out_keys / out_vals get int64 values or float64 bits, host[i] = 1
+// (and zeros in the outputs) when the host must parse the line
+__global__ void __launch_bounds__(256)
+k_tc_parse(const uint8_t *__restrict__ data, int64_t n, const int64_t *__restrict__ starts, int64_t nlines,
+           const uint8_t *__restrict__ sep, int32_t sep_len, int32_t key, int32_t value, int32_t key_kind,
+           int32_t value_kind, int64_t *__restrict__ out_keys, int64_t *__restrict__ out_vals, uint8_t *__restrict__ host) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nlines) return;
+    const int64_t b = starts[i];
+    const int64_t e = i + 1 < nlines ? starts[i + 1] - 1 : (data[n - 1] == '\n' ? n - 1 : n);
+    int64_t k = 0, v = 0;
+    const bool ok = tc_line(data, b, e, sep, sep_len, key, value, key_kind, value_kind, g_tc_pow5, &k, &v);
+    out_keys[i] = ok ? k : 0;
+    out_vals[i] = ok ? v : 0;
+    host[i] = ok ? 0 : 1;
+}
+
 // out[out_off[i] .. out_off[i] + lens[row]) = data[starts[row] ..), row = idx ? idx[i] : i  (token bytes made contiguous:
 // the (data, offsets) form dpk_hash_bytes / dpk_dict_encode take; or the bytes of the distinct keys for the host)
 __global__ void __launch_bounds__(256)
@@ -232,6 +302,43 @@ int dpk_tokenize_utf8_emit(const uint8_t *data, int64_t n, const int64_t *block_
     if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
     cudaStream_t st = (cudaStream_t)stream;
     DPK_LAUNCH("tok8_emit", st, k_tok8_emit<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_base, starts, lens));
+    return DPK_OK;
+}
+
+int dpk_textcols_count(const uint8_t *data, int64_t n, int64_t *block_counts, int64_t *flags, dpk_stream_t stream) {
+    if (n < 0) return fail(DPK_ERR_INVALID, "n=%lld < 0", (long long)n);
+    if (n == 0) return DPK_OK;
+    if (!data || !block_counts || !flags) return fail(DPK_ERR_INVALID, "NULL pointer");
+    const int64_t nb = dpk_tokenize_blocks(n);
+    if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
+    cudaStream_t st = (cudaStream_t)stream;
+    DPK_LAUNCH("tc_count", st, k_tc_count<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_counts, (unsigned long long *)flags));
+    return DPK_OK;
+}
+
+int dpk_textcols_emit(const uint8_t *data, int64_t n, const int64_t *block_base, int64_t *starts, dpk_stream_t stream) {
+    if (n < 0) return fail(DPK_ERR_INVALID, "n=%lld < 0", (long long)n);
+    if (n == 0) return DPK_OK;
+    if (!data || !block_base || !starts) return fail(DPK_ERR_INVALID, "NULL pointer");
+    const int64_t nb = dpk_tokenize_blocks(n);
+    if (nb >= ((int64_t)1 << 31)) return fail(DPK_ERR_INVALID, "text of %lld bytes is too long for one launch", (long long)n);
+    cudaStream_t st = (cudaStream_t)stream;
+    DPK_LAUNCH("tc_emit", st, k_tc_emit<<<(int)nb, TK_THREADS, 0, st>>>(data, n, block_base, starts));
+    return DPK_OK;
+}
+
+int dpk_textcols_parse(const uint8_t *data, int64_t n, const int64_t *starts, int64_t nlines, const uint8_t *sep,
+                       int32_t sep_len, int32_t key, int32_t value, int32_t key_kind, int32_t value_kind,
+                       int64_t *out_keys, int64_t *out_vals, uint8_t *host, dpk_stream_t stream) {
+    if (n < 0 || nlines < 0 || nlines > n) return fail(DPK_ERR_INVALID, "n=%lld nlines=%lld", (long long)n, (long long)nlines);
+    if (sep_len < 0 || key < 0 || value < 0) return fail(DPK_ERR_INVALID, "sep_len=%d key=%d value=%d", sep_len, key, value);
+    if ((key_kind != DPK_K_I64 && key_kind != DPK_K_F64) || (value_kind != DPK_K_I64 && value_kind != DPK_K_F64))
+        return fail(DPK_ERR_UNSUPPORTED, "column kinds %d, %d (DPK_K_I64 / DPK_K_F64)", key_kind, value_kind);
+    if (nlines == 0) return DPK_OK;
+    if (!data || !starts || (sep_len && !sep) || !out_keys || !out_vals || !host) return fail(DPK_ERR_INVALID, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    DPK_LAUNCH("tc_parse", st, k_tc_parse<<<(unsigned)((nlines + 255) / 256), 256, 0, st>>>(
+        data, n, starts, nlines, sep, sep_len, key, value, key_kind, value_kind, out_keys, out_vals, host));
     return DPK_OK;
 }
 

@@ -6,8 +6,8 @@ bit for bit:
 
   1. the keys, converted as join._key_column converts them, go through the numeric group-by (grouping.group_row_ids)
      carrying their row ids: every key's ids in (split, position) order;
-  2. a key's run is cut where the split changes (dpk_tdigest_heads; a ColumnarRDD's splits are blocks of `per` rows, so
-     row r lies in split r // per): one segment per (key, split);
+  2. a key's run is cut where the split changes (dpk_tdigest_heads with per = 1 over each row's split, found by a
+     search of the splits' first rows): one segment per (key, split);
   3. every segment's digest, MergingDigest().update(values) + compress(), into compacted scratch of min(L, TD_CAP)
      centroids per segment (dpk_tdigest_build);
   4. per key the first segment's digest absorbs the others in split order, then quantile(pp / 100.) for every pp in p
@@ -38,8 +38,9 @@ def segment_digests(rdd, P, thresholds):
     n = int(keys.numel())
     ids = torch.arange(n, dtype=torch.int64, device=dev)
     gk, gs, ov, part_off = grouping.group_row_ids([keys], [ids], P, thresholds)
-    per = rdd.splits[0].end - rdd.splits[0].begin
-    head = nv.tdigest_heads(ov, gs, per)
+    # each row's split (splits may be uneven: ColumnarRDD bounds): a key's run is cut where it changes
+    begins = torch.tensor([sp.begin for sp in rdd.splits[1:]], dtype=torch.int64, device=dev)
+    head = nv.tdigest_heads(torch.searchsorted(begins, ov, right=True), gs, 1)
     seg_starts = torch.cat([head.nonzero().view(-1), gs[-1:]])
     seg_off = torch.zeros_like(seg_starts)
     torch.cumsum((seg_starts[1:] - seg_starts[:-1]).clamp_(max=TD_CAP), 0, out=seg_off[1:])

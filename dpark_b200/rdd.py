@@ -11,6 +11,7 @@ on the GPU through dpark_b200.shuffle -- there is no CPU shuffle.
 """
 import itertools
 import math
+import operator
 import os
 import random
 import shutil
@@ -691,7 +692,10 @@ class ColumnarRDD(RDD):
     enter without ever becoming Python tuples; a ShuffledRDD on top of it takes
     the columns as they are."""
 
-    def __init__(self, ctx, keys, vals, numSlices):
+    def __init__(self, ctx, keys, vals, numSlices, bounds=None):
+        """bounds: optional split row bounds, a non-decreasing int sequence from 0 to the row count -- split i holds
+        rows [bounds[i], bounds[i + 1]) and numSlices is not used.  Without it the rows are cut into numSlices
+        blocks of ceil(n / numSlices)."""
         RDD.__init__(self, ctx)
         import torch
         self.keys = keys if torch.is_tensor(keys) else torch.from_numpy(np.ascontiguousarray(keys))
@@ -700,12 +704,16 @@ class ColumnarRDD(RDD):
             raise DparkUserFatalError("ragged pair columns: %d keys, %d values"
                                       % (self.keys.numel(), self.vals.numel()))
         n = int(self.keys.numel())
-        k = max(1, min(n, numSlices)) if n else 1
-        per = -(-n // k) if n else 0
+        if bounds is not None:
+            cuts = _split_bounds(bounds, n)
+        else:
+            k = max(1, min(n, numSlices)) if n else 1
+            per = -(-n // k) if n else 0
+            cuts = [min(n, i * per) for i in range(k)] + [min(n, k * per)]
         self._splits = []
-        for i in range(k):
+        for i in range(len(cuts) - 1):
             sp = Split(i)
-            sp.begin, sp.end = min(n, i * per), min(n, i * per + per)
+            sp.begin, sp.end = cuts[i], cuts[i + 1]
             self._splits.append(sp)
 
     def columns(self, split):
@@ -714,6 +722,19 @@ class ColumnarRDD(RDD):
     def compute(self, split):
         k, v = self.columns(split)
         return zip(k.cpu().tolist(), v.cpu().tolist())
+
+
+def _split_bounds(bounds, n):
+    try:
+        cuts = list(bounds)
+        if any(isinstance(b, bool) for b in cuts):
+            raise TypeError("bool")
+        cuts = [operator.index(b) for b in cuts]
+    except TypeError:
+        raise DparkUserFatalError("split bounds must be a sequence of ints, got %r" % (bounds,))
+    if not cuts or cuts[0] != 0 or cuts[-1] != n or any(a > b for a, b in zip(cuts, cuts[1:])):
+        raise DparkUserFatalError("split bounds must rise from 0 to %d without decreasing, got %r" % (n, cuts))
+    return cuts
 
 
 def device_path_applies(rdds, max_rows=None):

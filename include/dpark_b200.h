@@ -494,6 +494,25 @@ int dpk_tokenize_utf8_count(const uint8_t *data, int64_t n, int64_t *block_count
 int dpk_tokenize_utf8_emit(const uint8_t *data, int64_t n, const int64_t *block_base, int64_t *starts, int64_t *lens,
                            dpk_stream_t stream);
 
+/* ---- f10: numeric text columns (DparkContext.textFileColumns) ---------------------------------------------------------
+ * A byte range that starts on a line start; a line ends at the next '\n' or at n, and a final '\n' opens no line.
+ *   dpk_textcols_count : per dpk_tokenize_blocks(n) block of 4096 bytes its number of line starts; ORs bit 0 into
+ *                        *flags when a byte >= 0x80 occurs (the caller then checks the range with
+ *                        dpk_tokenize_utf8_count).
+ *   dpk_textcols_emit  : takes the EXCLUSIVE scan of those counts and writes every line start, in text order.
+ *   dpk_textcols_parse : per line, fields key and value of line.split() (sep_len == 0) or line.split(sep) (sep[sep_len]
+ *                        bytes, UTF-8) parsed as int() (kind DPK_K_I64: out = the int64) or float() (DPK_K_F64: out =
+ *                        the float64 bits).  Only [+-]?[0-9]{1,19} within int64, and decimal / exponent / inf /
+ *                        infinity / nan ASCII floats whose rounding the conversion decides, with \t \n \v \f \r and
+ *                        space stripped, are parsed here; every other line gets host[i] = 1 and zeros, and the caller
+ *                        must parse it with Python.
+ * None allocates or synchronises. */
+int dpk_textcols_count(const uint8_t *data, int64_t n, int64_t *block_counts, int64_t *flags, dpk_stream_t stream);
+int dpk_textcols_emit(const uint8_t *data, int64_t n, const int64_t *block_base, int64_t *starts, dpk_stream_t stream);
+int dpk_textcols_parse(const uint8_t *data, int64_t n, const int64_t *starts, int64_t nlines, const uint8_t *sep,
+                       int32_t sep_len, int32_t key, int32_t value, int32_t key_kind, int32_t value_kind,
+                       int64_t *out_keys, int64_t *out_vals, uint8_t *host, dpk_stream_t stream);
+
 /* ---- variable-length keys (str / bytes): key identity on the device ---------
  * The reference's dicts compare keys by value; two different strings may share
  * a portable_hash, so the hash alone cannot be the key.  dpk_dict_encode gives
