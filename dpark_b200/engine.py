@@ -227,7 +227,10 @@ def _key_kind_of(splits):
 
 def _run_reduce(splits, P, thr, op, dev):
     res = ShuffleResult(P)
-    tensor_in = splits and not isinstance(splits[0], columnar.Columns)
+    if not splits:                  # a parent without splits (an empty file): P empty partitions, as group_by_key gives
+        res.parts = [([], []) for _ in range(P)]
+        return res
+    tensor_in = not isinstance(splits[0], columnar.Columns)
     if tensor_in:
         from . import join
         kc = [k.to(dev).contiguous() for k, v in splits]

@@ -87,7 +87,7 @@ def bernoulli(ranges, nrows, frac, seed):
     rng = torch.tensor(ranges, dtype=torch.int64).view(len(ranges), 2).to(dev)
     ids, counts = nv.sample_bernoulli(states, rng, _frac_arg(frac), nrows)
     counts = counts.cpu().tolist()
-    return torch.cat([ids[b:b + c] for (b, _), c in zip(ranges, counts)]), counts
+    return torch.cat([ids[:0]] + [ids[b:b + c] for (b, _), c in zip(ranges, counts)]), counts
 
 
 def _refold_first(digests):

@@ -53,8 +53,8 @@ def device_sort_applies(rdd, key):
 
 def sample_bounds(rdd, key, reverse, numSplits):
     """RDD.sort's range bounds over rdd, from the same samples the composition takes (the first n rows of every split,
-    mapped by key), read from column slices instead of through compute.  [] for a single split."""
-    if len(rdd) == 1:
+    mapped by key), read from column slices instead of through compute.  [] for a single split or none."""
+    if len(rdd) <= 1:
         return []
     if numSplits is None:
         numSplits = min(rdd.ctx.defaultMinSplits, len(rdd))
@@ -121,7 +121,8 @@ class ColumnarSortedRDD(DeviceResultRDD):
         self.taskMemory, self.sort_rddconf = taskMemory, rddconf
         self.order = order_of(key)
         self.bounds = sample_bounds(parent, key, reverse, numSplits)
-        self._splits = [Split(i) for i in range(len(self.bounds) + 1)]
+        # no partitions for an input without splits, as the composition returns that input itself
+        self._splits = [Split(i) for i in range(len(self.bounds) + 1)] if len(parent) else []
 
     def parents(self):
         return [self.parent]
