@@ -339,11 +339,25 @@ def check_counts(cnt_h):
                              "bits; the partition's result is invalid (dpk_combine out_counts = -1)")
 
 
+def nan_key_flag(keys):
+    """Device flag: the float key column holds a NaN (None for integer keys).  Read by check_nan_flag once the batch's
+    result sizes have been read back, so that no extra host sync is needed."""
+    return torch.isnan(keys).any() if keys.dtype.is_floating_point else None
+
+
+def check_nan_flag(flag):
+    """TypeError for NaN keys, as the engine raises (join.reject_nan_keys): CPython hashes NaN by identity, so every
+    NaN row is a key of its own there, while the device would merge NaNs with equal bits."""
+    if flag is not None and bool(flag):
+        raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
+
+
 class HostShuffle(object):
     """End-to-end reduceByKey for HOST-resident columns, one batch at a time: the serial form of
     HostShuffleStream (depth 1).  Per call: pinned host -> device copy of every map split, map_side,
     exchange, reduce_side, device -> pinned host copy of every partition's distinct (key, combined)
-    rows.  Buffers are allocated once and reused."""
+    rows.  Buffers are allocated once and reused: the views run() returns are valid until the next run().
+    Float keys holding a NaN raise TypeError."""
 
     def __init__(self, n_rows, key_dtype, val_dtype, P, op="sum", splits=8, thresholds=None, group=None,
                  device=None, sub_bits=None, world=1, peer_exchange=None, map_combine=False):
@@ -373,6 +387,7 @@ class HostShuffle(object):
             self.d_vals[a:b].copy_(self.h_vals[a:b], non_blocking=True)
             kc.append(self.d_keys[a:b])
             vc.append(self.d_vals[a:b])
+        nan = nan_key_flag(self.d_keys)
         px = self.peer_exchange
         if px is not None and px.mode == "fused" and not self.map_combine:
             from . import peer                 # the scatter kernel stores straight into peer memory
@@ -391,6 +406,7 @@ class HostShuffle(object):
         check_counts(cnt_h)
         if px is not None:
             px.check()
+        check_nan_flag(nan)
         nout = sum(cnt_h)
         if self.out_keys is None or self.out_keys.numel() < nout:
             self.out_keys = torch.empty(max(nout, 1), dtype=ok.dtype).pin_memory()
@@ -422,6 +438,14 @@ class HostShuffleStream(object):
     reduce: [(partition, keys, combined values)]; group: [(partition, group keys, group starts, values)] with the
     values of group g at values[starts[g]:starts[g+1]] in (map split, position) order.  All pinned-host views of the
     slot's output buffers: valid until that slot is collected again (`depth - 1` further collect() calls).
+
+    Result dtypes.  reduce: keys in the key dtype, values in nv.acc_dtype (int64 or float64).  group: keys int64 for
+    integer keys and float64 for float keys (int32 and float32 keys are widened on the device, as the engine's
+    group-by does; -0.0 and 0.0 are one key, spelled 0.0), values in the value dtype.
+
+    The copies of h_keys / h_vals run asynchronously on the slot's stream: the caller may rewrite them once that
+    batch's collect() has returned, not before.  Float keys holding a NaN make that collect() raise TypeError (the
+    slot is free again afterwards).
     """
 
     class _Slot(object):
@@ -441,19 +465,25 @@ class HostShuffleStream(object):
         ksz = torch.empty(0, dtype=key_dtype).element_size()
         vsz = torch.empty(0, dtype=val_dtype).element_size()
         out_vdt = nv.acc_dtype(val_dtype) if kind == "reduce" else val_dtype
+        # group: the radix sort orders int64 key bits, so keys go in widened (float keys as canonical float64)
+        wide_kdt = torch.float64 if key_dtype.is_floating_point else torch.int64
+        out_kdt = key_dtype if kind == "reduce" else wide_kdt
         self.slots = []
         for _ in range(depth):
             s = self._Slot()
             s.stream = torch.cuda.Stream(device=self.device)
             s.d_keys = torch.empty(n_rows, dtype=key_dtype, device=self.device)
             s.d_vals = torch.empty(n_rows, dtype=val_dtype, device=self.device)
-            s.out_keys = torch.empty(cap, dtype=key_dtype if kind == "reduce" else torch.int64).pin_memory()
+            s.d_wide = None
+            if kind == "group" and key_dtype != wide_kdt:
+                s.d_wide = torch.empty(n_rows, dtype=wide_kdt, device=self.device)
+            s.out_keys = torch.empty(cap, dtype=out_kdt).pin_memory()
             s.out_vals = torch.empty(cap, dtype=out_vdt).pin_memory()
             s.out_starts = torch.empty(cap + 1, dtype=torch.int64).pin_memory() if kind == "group" else None
             s.px = None
             if self.world > 1 and peer_mode is not None:
                 from . import peer
-                s.px = peer.PeerExchange(cap, key_dtype, val_dtype, self.device, group=group, mode="push")
+                s.px = peer.PeerExchange(cap, out_kdt, val_dtype, self.device, group=group, mode="push")
             s.busy = False
             self.slots.append(s)
         self.next_submit = 0
@@ -467,14 +497,21 @@ class HostShuffleStream(object):
             raise RuntimeError("all %d slots are in flight: collect() first" % len(self.slots))
         self.next_submit += 1
         per = (self.n + self.splits - 1) // self.splits
+        bounds = [(min(self.n, i * per), min(self.n, (i + 1) * per)) for i in range(self.splits)]
         with torch.cuda.stream(s.stream):
-            kc, vc = [], []
-            for i in range(self.splits):
-                a, b = min(self.n, i * per), min(self.n, (i + 1) * per)
+            for a, b in bounds:
                 s.d_keys[a:b].copy_(h_keys[a:b], non_blocking=True)
                 s.d_vals[a:b].copy_(h_vals[a:b], non_blocking=True)
-                kc.append(s.d_keys[a:b])
-                vc.append(s.d_vals[a:b])
+            s.nan = nan_key_flag(s.d_keys)
+            keys = s.d_keys
+            if self.kind == "group":
+                if s.d_wide is not None:
+                    keys = s.d_wide
+                    keys.copy_(s.d_keys)
+                if keys.dtype.is_floating_point:
+                    keys.add_(0.0)             # -0.0 and 0.0 are one key, spelled 0.0
+            kc = [keys[a:b] for a, b in bounds]
+            vc = [s.d_vals[a:b] for a, b in bounds]
             mo = map_side(kc, vc, self.P, self.thresholds, False, self.sub_bits, unordered=self.kind == "reduce")
             if s.px is not None:
                 from . import peer
@@ -493,13 +530,16 @@ class HostShuffleStream(object):
         if not s.busy:
             raise RuntimeError("nothing in flight")
         self.next_collect += 1
-        with torch.cuda.stream(s.stream):
-            res = self._collect_reduce(s) if self.kind == "reduce" else self._collect_group(s)
-            s.stream.synchronize()
-            if s.px is not None:
-                s.px.check()
-        s.result = None
-        s.busy = False
+        try:
+            with torch.cuda.stream(s.stream):
+                res = self._collect_reduce(s) if self.kind == "reduce" else self._collect_group(s)
+                s.stream.synchronize()
+                if s.px is not None:
+                    s.px.check()
+            check_nan_flag(s.nan)
+        finally:
+            s.result = None
+            s.busy = False
         return res
 
     def _collect_reduce(self, s):
@@ -521,7 +561,7 @@ class HostShuffleStream(object):
         G = int(ng.item())                                           # waits for THIS batch only
         off_h = off.cpu().tolist()
         nval = int(ov.numel())
-        s.out_keys[:G].copy_(gk[:G], non_blocking=True)
+        s.out_keys[:G].copy_(gk[:G].view(s.out_keys.dtype), non_blocking=True)
         s.out_starts[:G + 1].copy_(gs[:G + 1], non_blocking=True)
         s.out_vals[:nval].copy_(ov, non_blocking=True)
         s.stream.synchronize()
