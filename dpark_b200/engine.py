@@ -134,39 +134,57 @@ def _run_shuffle_spmd(srdd, rank, world):
         splits = _gather_parent(srdd, numeric, only=mine)
     blocks = shuffle.owner_blocks(P, world)
     tensor_in = bool(splits) and not isinstance(splits[0], columnar.Columns)
-    # what every rank must agree on before any collective: key kind, value kinds
+    # what every rank must agree on before any collective: key kind, value kinds, and what the one-process checks
+    # read from the whole input (NaN keys of columns; the terms of the int64 sum bound, in split order)
     if tensor_in:
-        desc = ("tensor", str(splits[0][0].dtype), str(splits[0][1].dtype))
+        kc = [k.to(dev).contiguous() for k, v in splits]
+        from . import join
+        desc = ("tensor", str(splits[0][0].dtype), str(splits[0][1].dtype), join.has_nan_key(kc))
     else:
-        desc = ("cols", sorted(set(c.key_kind for c in splits if c.n)), sorted(set(c.val_kind for c in splits if c.n)))
+        desc = ("cols", sorted(set(c.key_kind for c in splits if c.n)), sorted(set(c.val_kind for c in splits if c.n)),
+                _int_sum_terms(splits) if numeric and srdd.op == "sum" else [])
     descs = spmd.all_gather_objects(desc)
-    res = ShuffleResult(P)
     if any(d[0] == "tensor" for d in descs):
         if not all(d[0] == "tensor" or d[1] == [] for d in descs):
             raise TypeError("mixed columnar and row inputs in one shuffle are not supported on the GPU path")
+        from . import join
+        join.reject_nan_keys((), flag=any(d[0] == "tensor" and d[3] for d in descs))
         kd = next(d for d in descs if d[0] == "tensor")
         kdt, vdt = getattr(torch, kd[1].split(".")[1]), getattr(torch, kd[2].split(".")[1])
-        kc = [k.to(dev).contiguous() for k, v in splits] or [torch.empty(0, dtype=kdt, device=dev)]
-        vc = [v.to(dev).contiguous() for k, v in splits] or [torch.empty(0, dtype=vdt, device=dev)]
-        owned = _device_reduce(kc, vc, P, thr, srdd.op, world)
-    else:
-        kinds = sorted(set(k for d in descs for k in d[1]))
-        vkinds = sorted(set(k for d in descs for k in d[2]))
-        if len(kinds) > 1:
-            raise TypeError("mixed key types %s in one shuffle are not supported on the GPU path" % kinds)
-        kk = kinds[0] if kinds else columnar.KEY_I64
-        if numeric and len(vkinds) > 1:
+        kc = kc if tensor_in else [torch.empty(0, dtype=kdt, device=dev)]
+        vc = [v.to(dev).contiguous() for k, v in splits] if tensor_in else [torch.empty(0, dtype=vdt, device=dev)]
+        return _gathered(_device_reduce(kc, vc, P, thr, srdd.op, world), P)
+    kinds = sorted(set(k for d in descs for k in d[1]))
+    vkinds = set(k for d in descs for k in d[2])
+    if len(kinds) > 1:
+        raise TypeError("mixed key types %s in one shuffle are not supported on the GPU path" % kinds)
+    kk = kinds[0] if kinds else columnar.KEY_I64
+    if numeric:
+        if len(vkinds) > 1:
             raise TypeError("reduceByKey values must be all int or all float on the GPU path")
-        if numeric and kk in (columnar.KEY_I64, columnar.KEY_F64) and not ROUTE_EVERYTHING:
+        _check_int_sum_range((), vkinds, srdd.op, terms=[t for d in descs for t in d[3]])
+    if numeric and kk in (columnar.KEY_I64, columnar.KEY_F64) and not ROUTE_EVERYTHING:
+        def reduce_all(cols, vdt, op):
             kdt = np.int64 if kk == columnar.KEY_I64 else np.float64
-            vdt = torch.float64 if vkinds == [columnar.VAL_F64] else torch.int64
-            kc = [torch.from_numpy(c.keys.astype(kdt, copy=False)).to(dev) for c in splits] or \
+            kc = [torch.from_numpy(c.keys.astype(kdt, copy=False)).to(dev) for c in cols] or \
                 [torch.empty(0, dtype=torch.int64 if kk == columnar.KEY_I64 else torch.float64, device=dev)]
-            vc = [torch.from_numpy(c.vals).to(dev).to(vdt) for c in splits] or [torch.empty(0, dtype=vdt, device=dev)]
-            owned = _device_reduce(kc, vc, P, thr, srdd.op, world)
-        else:
-            owned = _routed_shuffle(splits, kk, numeric, P, thr, srdd.op, dev, rank, world, blocks)
-    for part in spmd.all_gather_objects(owned):
+            vc = [torch.from_numpy(c.vals).to(dev).to(vdt) for c in cols] or [torch.empty(0, dtype=vdt, device=dev)]
+            return _gathered(_device_reduce(kc, vc, P, thr, op, world), P)
+        _check_int_prod_range(splits, vkinds, srdd.op, lambda logs: reduce_all(logs, torch.float64, "sum"))
+        return reduce_all(splits, torch.float64 if vkinds == {columnar.VAL_F64} else torch.int64, srdd.op)
+    return _gathered(_routed_shuffle(splits, kk, numeric, P, thr, srdd.op, dev, rank, world, blocks), P)
+
+
+def _gathered(owned, P):
+    """Every rank's {partition: columns} -> the ShuffleResult of all P partitions, on every rank.  A rank may hand in
+    the exception its owner stage raised instead: every rank raises the first one, in rank order."""
+    from . import spmd
+    res = ShuffleResult(P)
+    parts = spmd.all_gather_objects(owned)
+    for part in parts:
+        if isinstance(part, Exception):
+            raise part
+    for part in parts:
         for p, cols in part.items():
             res.parts[p] = cols
     for p in range(P):
@@ -210,11 +228,14 @@ def _routed_shuffle(splits, kk, numeric, P, thr, op, dev, rank, world, blocks):
             per_dest[d][1].extend(vals[i] for i in idx)
     got = spmd.all_to_all_objects(per_dest)
     local = [columnar.ingest_pairs(zip(ks, vs), "shuffle", numeric) for ks, vs in got]
-    with shuffle.local_only():
-        if numeric:
-            r = _run_reduce(local, P, thr, op, dev)
-        else:
-            r = _run_group(local, P, thr, dev)
+    try:
+        with shuffle.local_only():
+            if numeric:
+                r = _run_reduce(local, P, thr, op, dev)
+            else:
+                r = _run_group(local, P, thr, dev)
+    except Exception as e:      # raised on this owner alone (the int64 product check of its keys): _gathered raises
+        return e                # it on every rank instead of leaving the others waiting in the next collective
     return {p: r.parts[p] for p in range(blocks[rank], blocks[rank + 1])}
 
 
@@ -261,14 +282,21 @@ def _run_reduce(splits, P, thr, op, dev):
     return strings.reduce_by_key_bytes(splits, kk, P, thr, op, dev, res)
 
 
-def _check_int_sum_range(splits, vkinds, op):
+def _int_sum_terms(splits):
+    """The terms of _check_int_sum_range: sum |v| of each split, in split order."""
+    return [float(np.abs(c.vals.astype(np.float64)).sum()) for c in splits if c.n]
+
+
+def _check_int_sum_range(splits, vkinds, op, terms=None):
     """The reference adds Python big ints; the device accumulates in int64.  A cheap sufficient check on the ingested
-    columns: if the sum of |v| over the whole shuffle stays below 2^63 no key's sum can wrap."""
+    columns: if the sum of |v| over the whole shuffle stays below 2^63 no key's sum can wrap.  terms: the
+    _int_sum_terms of every split of a distributed shuffle, gathered from the ranks in split order (splits is then
+    not read), so that every rank adds the same terms in the same order as one process does."""
     if vkinds == {columnar.VAL_I64} and op == "sum":
-        bound = sum(float(np.abs(c.vals.astype(np.float64)).sum()) for c in splits if c.n)
+        bound = sum(_int_sum_terms(splits) if terms is None else terms)
         if bound >= 2.0 ** 63:
-            raise OverflowError("reduceByKey(add): the values' magnitudes sum to %.3g >= 2^63; int64 accumulation on the "
-                                "GPU path could wrap where the reference's big ints do not" % bound)
+            raise OverflowError("reduceByKey(add): the values' magnitudes sum to %.3g >= 2^63; int64 accumulation on "
+                                "the GPU path could wrap where the reference's big ints do not" % bound)
 
 
 PROD_LOG2_LIMIT = 63 - 1e-9

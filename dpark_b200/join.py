@@ -30,12 +30,16 @@ from . import grouping
 from .rdd import DeviceResultRDD, Split, device_path_applies
 
 
-def reject_nan_keys(key_columns):
+def has_nan_key(key_columns):
+    return any(k.dtype.is_floating_point and bool(torch.isnan(k).any()) for k in key_columns)
+
+
+def reject_nan_keys(key_columns, flag=None):
     """TypeError if a float key column holds a NaN, as the row path's ingest raises (columnar._key_column): CPython
-    hashes NaN by identity, so every NaN row is a key of its own there, while the device would merge equal bits."""
-    for k in key_columns:
-        if k.dtype.is_floating_point and bool(torch.isnan(k).any()):
-            raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
+    hashes NaN by identity, so every NaN row is a key of its own there, while the device would merge equal bits.
+    flag: has_nan_key already evaluated (under torch.distributed: over every rank's columns, so all ranks agree)."""
+    if has_nan_key(key_columns) if flag is None else flag:
+        raise TypeError("NaN keys are not supported (CPython hashes NaN by identity)")
 
 
 def _key_column(rdds, dev):

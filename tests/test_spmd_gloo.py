@@ -98,7 +98,27 @@ def _job(dc):
     return out
 
 
-def _worker(rank, world, port, out_q):
+def _outcome(f):
+    try:
+        return ("ok", f())
+    except Exception as e:
+        return (type(e).__name__, str(e))
+
+
+def _agreed_checks_job(dc):
+    """The checks one process makes over the whole input, where no rank's own splits fail them: the int64 sum bound
+    (rank 0 holds 2^62 + 1, rank 1 holds 2^62 + 2^62) and a NaN key of a ColumnarRDD in rank 1's split.  Both are
+    decided from the descriptors every rank all-gathers before the first collective, so no device stage runs."""
+    import numpy as np
+    import operator
+    from dpark_b200.rdd import ColumnarRDD
+    rows = [(7, 2 ** 62), (8, 1), (7, 2 ** 62), (7, 2 ** 62)]
+    cols = ColumnarRDD(dc, np.array([1.0, 2.0, 3.0, np.nan]), np.arange(4, dtype=np.int64), 0, bounds=[0, 2, 4])
+    return {"sum": _outcome(lambda: dc.parallelize(rows, 2).reduceByKey(operator.add, 3).collect()),
+            "nan": _outcome(lambda: cols.reduceByKey(operator.add, 2).collect())}
+
+
+def _worker(rank, world, port, out_q, job="_job"):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     sys.argv = [sys.argv[0]]
     if world > 1:
@@ -106,7 +126,7 @@ def _worker(rank, world, port, out_q):
     try:
         _patch_gpu_stages()
         from dpark_b200 import DparkContext
-        out_q.put((rank, _job(DparkContext("local"))))
+        out_q.put((rank, globals()[job](DparkContext("local"))))
     except Exception as e:                      # surface the failure instead of leaving the other rank waiting
         import traceback
         out_q.put((rank, {"error": "%s\n%s" % (e, traceback.format_exc())}))
@@ -115,11 +135,11 @@ def _worker(rank, world, port, out_q):
             dist.destroy_process_group()
 
 
-def _run(world):
+def _run(world, job="_job"):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
+    procs = [ctx.Process(target=_worker, args=(r, world, port, q, job)) for r in range(world)]
     for p in procs:
         p.start()
     got = dict(q.get(timeout=120) for _ in range(world))
@@ -136,3 +156,16 @@ def test_two_driver_processes_see_what_one_process_computes():
     assert one["acc"] == 400 and one["wc"] and one["group"] and one["join"] and len(one["pagerank"]) == 12
     for rank in (0, 1):
         assert two[rank] == one, "rank %d diverged" % rank
+
+
+def test_whole_input_checks_are_agreed_by_every_rank():
+    from dpark_b200 import columnar, engine
+    with pytest.raises(OverflowError) as big:          # one process, over both splits
+        engine._check_int_sum_range([columnar.ingest_pairs([(7, 2 ** 62), (8, 1)]),
+                                     columnar.ingest_pairs([(7, 2 ** 62), (7, 2 ** 62)])], {columnar.VAL_I64}, "sum")
+    want = {"sum": ("OverflowError", str(big.value)),
+            "nan": ("TypeError", "NaN keys are not supported (CPython hashes NaN by identity)")}
+    two = _run(2, "_agreed_checks_job")
+    for rank in (0, 1):
+        assert "error" not in two[rank], two[rank]["error"]
+        assert two[rank] == want, "rank %d" % rank
